@@ -3,7 +3,7 @@
 NVCC      ?= /usr/local/cuda/bin/nvcc
 HOSTCC    := $(shell [ -x /usr/bin/gcc ] && echo /usr/bin/gcc || echo gcc)
 OMPFLAG   := $(shell echo 'int main(){return 0;}' | $(HOSTCC) -fopenmp -x c - -o /dev/null 2>/dev/null && echo -fopenmp)
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVCCFLAGS := -O3 -std=c++17 -lineinfo $(ARCH) -Xcompiler -fPIC -Xptxas -v --expt-relaxed-constexpr
 CSRC      := dg-mesh_b200/csrc
 LIB       := dg-mesh_b200/libdgmesh_b200.so

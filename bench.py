@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """bench.py -- the headline benchmark of BASELINE.json:
-raster fwd+bwd frames/s @ 100k Gaussians, 800x800 (configs[1], SURVEY.md 8(d) C2), 1/2/4/8 B200.
+raster fwd+bwd frames/s @ 100k Gaussians, 800x800 (configs[1], SURVEY.md 8(d) C2), 1/2/4/8 H100.
 
   python bench.py --gpus N --steps K --warmup W            # this repo (CUDA path via the C-ABI)
   python bench.py --impl reference --gpus N --steps K ...  # stock diff_gaussian_rasterization (oracle/_ref)
+  python bench.py ... --dump-outputs DIR                    # + the last timed step's outputs as DIR/<name>.npy
 
 A "step" is one batch of 8 training frames of a DYNAMIC scene (8 cameras on a ring at times
 t_k = k/8, SURVEY C4): every frame renders the canonical Gaussians deformed for its own time --
@@ -101,8 +102,8 @@ class Exchange:
         self.kind, self.handle, self.epoch = "nccl", None, 1
         n_pad = (n + 3) // 4 * 4
         self.buf = None
-        # measured (profiles/r2_nvls_n2.json, r2_nvls_n8.json): on 8 GPUs our kernel beats ncclAllReduce 1.3-1.5x, on 2
-        # GPUs NCCL's direct peer copy moves less data than a multicast round trip and wins (0.066 vs 0.094 ms)
+        # on 2 GPUs NCCL's direct peer copy moves less data than a multicast round trip; from 4 GPUs on the
+        # multicast exchange sends and receives the buffer once per GPU
         default = "nvls" if world >= 4 else "nccl"
         if world > 1 and os.environ.get("DGMESH_B200_EXCHANGE", default) == "nvls":
             try:
@@ -114,7 +115,7 @@ class Exchange:
                 buf.zero_()
                 h.barrier()
                 self.buf, self.handle, self.kind = buf, h, "nvls (own kernel, multimem.ld_reduce / multimem.st)"
-                self.blocks = 296   # dp.NvlsFlatGrad.BLOCKS
+                self.blocks = dp_blocks()
             except Exception as e:  # recorded in the JSON line
                 self.kind = f"nccl (nvls unavailable: {type(e).__name__}: {e})"
         if world > 1:
@@ -139,6 +140,27 @@ class Exchange:
                                                _dgm_lib.stream_ptr())
         _dgm_lib.check(rc, "dgx_allreduce_nvls")
         self.epoch += 2
+
+
+def dp_blocks():
+    import dp
+    return dp.NvlsFlatGrad.BLOCKS
+
+
+DUMP_COLOR_SAMPLES = 4_000_000   # rendered values kept by --dump-outputs (16 MB of the 61 MB batch)
+
+
+def dump_outputs(out_dir, color, leaves):
+    """What the timed path hands its caller after its last step: the rendered batch (the values at a fixed, seeded
+    sample of flat positions) and the gradient of every Gaussian parameter, as float32 .npy files."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    flat = color.detach().reshape(-1)
+    g = torch.Generator().manual_seed(123)
+    idx = torch.randperm(flat.numel(), generator=g)[:min(DUMP_COLOR_SAMPLES, flat.numel())].sort().values
+    np.save(os.path.join(out_dir, "color_sample.npy"), flat[idx.to(flat.device)].float().cpu().numpy())
+    for n, p in leaves.items():
+        np.save(os.path.join(out_dir, f"grad_{n}.npy"), p.grad.detach().float().cpu().numpy())
 
 
 def flat_params(sc, device, world=1):
@@ -395,6 +417,9 @@ def main():
                          "not used with NCCL: capturing the all-reduce hung in this round's test")
     ap.add_argument("--no-train-step", action="store_true",
                     help="skip the full-train-step leg (BASELINE.json's second metric, N=1 only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (rendered colours, sampled; "
+                         "parameter gradients) as DIR/<name>.npy (rank 0)")
     a = ap.parse_args()
     a.warmup = max(a.warmup, 3)
     # exactly ONE line may reach stdout (the JSON): libraries that print there (NCCL's version banner)
@@ -445,14 +470,16 @@ def main():
     # which is the shorter host path (measured at N = 8: 0.541 vs 0.577 ms per step)
     one = ours and len(my_frames) == 1
 
+    last = {}   # the colour of the step's last render (a graph replay rewrites the captured tensor in place)
+
     def step():
         gflat.zero_()
         if one:
-            run_frames(dgr, synth, leaves, cams, dpix, bg, my_frames, deltas=deltas_all)
+            last["color"] = run_frames(dgr, synth, leaves, cams, dpix, bg, my_frames, deltas=deltas_all)
         elif ours:
-            run_batch(dgr, leaves, dev_settings, dpix_stacked, deltas=my_deltas)
+            last["color"] = run_batch(dgr, leaves, dev_settings, dpix_stacked, deltas=my_deltas)
         else:
-            run_frames(dgr, synth, leaves, cams, dpix, bg, my_frames, deltas=deltas_all)
+            last["color"] = run_frames(dgr, synth, leaves, cams, dpix, bg, my_frames, deltas=deltas_all)
         if world > 1:
             exchange.allreduce()  # the one collective of the step (SURVEY 8(e))
 
@@ -501,6 +528,8 @@ def main():
         sampler.start()
     ms = timed(timed_step, a.steps, a.warmup, world)
     clocks = sampler.stop() if rank == 0 else None
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, last["color"], leaves)
     if use_graph:
         # graph replay cannot wait for the status words (no host interaction inside a graph): prove that no frame
         # overflowed its instance workspace by comparing the replayed gradient with an eager step's
@@ -588,7 +617,7 @@ def main():
                           else "GaussianRasterizer per frame (reference API)",
                    "l2_policy": "inputs larger than L2: per step 8 frames x (~42 MB instance records + 12 MB "
                                 "per-Gaussian state + 13 MB pixel state) + 24 MB parameters + 61 MB pixel "
-                                "gradients = ~620 MB streamed through the 126 MB L2"},
+                                "gradients = ~620 MB streamed through the 50 MB L2"},
         "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
         "clocks": clocks,
     }
@@ -604,7 +633,7 @@ def main():
         out["gpu_launches"] = 0
         out["cpu_baseline"] = {"value": value, "unit": "frames/s", "cores": os.cpu_count(), "kind": "reference",
                                "sample": "stock diff_gaussian_rasterization (unmodified reference sources built for "
-                                         "sm_100) on ONE B200, same 8-frame batch; host threads only launch kernels"}
+                                         "sm_90a) on ONE H100, same 8-frame batch; host threads only launch kernels"}
         out["e2e"] = {"value": value, "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
         out["e2e_host_buffers"] = {"value": e2e_value, "unit": "frames/s"}
     else:
@@ -643,7 +672,7 @@ def main():
         if os.path.exists(peaks_path):
             peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         else:
-            peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+            peak, peak_src = 3350.0, "H100 SXM data sheet (HBM3, 700 W card)"
         achieved = alg[dom] / (kern_ms[dom] * 1e-3) / 1e9
         traffic = None
         tp = os.path.join(ROOT, "profiles", "traffic.json")

@@ -1,4 +1,4 @@
-"""dgmesh_b200 -- B200-native (sm_100a) implementation of DG-Mesh's per-iteration hot path.
+"""dgmesh_b200 -- H100-native (sm_90a) implementation of DG-Mesh's per-iteration hot path.
 
 The package holds the CUDA kernels + C-ABI (`csrc/`, `libdgmesh_b200.so`) and the
 host-side mirrors of the reference's Python surface for this path:

@@ -32,9 +32,8 @@ int bad(const char* msg) {
 namespace dgm {
 Profiler g_prof;
 // programmatic dependent launch between the rasterizer's kernels: DGMESH_B200_PDL=1 turns it on.
-// Off by default: measured on B200 (profiles/r2_pdl_ab.json) it is 2-3 % SLOWER for this chain --
-// early-resident dependents hold CTA slots / shared memory while the predecessor's tail is still
-// running, and the launch gaps it could hide total only ~30 us of a 440 us frame.
+// Off by default: early-resident dependents hold CTA slots / shared memory while the predecessor's
+// tail is still running, and the launch gaps it could hide are a small part of a frame.
 int g_pdl = [] {
   const char* e = getenv("DGMESH_B200_PDL");
   return (e && e[0] == '1') ? 1 : 0;
@@ -85,7 +84,7 @@ cudaError_t launch_export_state(int P, int W, int H, int64_t R_cap, const void* 
 
 extern "C" {
 
-const char* dgm_version(void) { return "dgmesh_b200 0.1 sm_100a"; }
+const char* dgm_version(void) { return "dgmesh_b200 0.1 sm_90a"; }
 const char* dgm_last_error(void) { return g_last_error; }
 
 int dgr_workspace_sizes(int P, int W, int H, int64_t R_cap, size_t* geom_bytes, size_t* binning_bytes,

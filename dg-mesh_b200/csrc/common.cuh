@@ -1,14 +1,14 @@
-// common.cuh -- shared device helpers + private workspace layouts (sm_100a only).
+// common.cuh -- shared device helpers + private workspace layouts (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stddef.h>
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "dgmesh_b200 is written for sm_100a (Blackwell B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 900)
+#error "dgmesh_b200 is written for sm_90a (Hopper H100)"
 #endif
 
-#define DGM_NUM_SMS 148          // B200: 2 dies x 74 SMs
+#define DGM_NUM_SMS 132          // H100 SXM
 #define TILE_X 16                // reference BLOCK_X / BLOCK_Y (dgr/cuda_rasterizer/config.h:16-17)
 #define TILE_Y 16
 #define TILE_PIX (TILE_X * TILE_Y)
@@ -156,6 +156,9 @@ __device__ __forceinline__ void pdl_launch() { asm volatile("griddepcontrol.laun
 __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d)
                : "memory");
+}
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {  // 8-byte aligned
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
 

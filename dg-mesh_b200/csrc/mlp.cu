@@ -1,4 +1,4 @@
-// mlp.cu -- deformation / appearance MLPs on the tcgen05 tensor cores.
+// mlp.cu -- deformation / appearance MLPs on the Hopper tensor cores (wgmma).
 //
 // The networks (dgmesh/utils/time_utils.py): DeformNetwork / DeformNetworkNormal /
 // DeformNetworkNormalSep / AppearanceNetwork share one trunk --
@@ -32,39 +32,64 @@ static int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_sms <= 0) g_sms = 148;
+    if (g_sms <= 0) g_sms = DGM_NUM_SMS;
   }
   return g_sms;
+}
+
+typedef void (*LayerKernel)(const LayerArgs);
+typedef void (*DwKernel)(const DwArgs);
+static LayerKernel layer_kernel(bool resident, int N) {
+  switch (N) {
+#define DGM_CASE(n) \
+  case n: return resident ? layer_gemm_kernel<true, n> : layer_gemm_kernel<false, n>;
+    DGM_GEMM_NS(DGM_CASE)
+#undef DGM_CASE
+  }
+  return nullptr;
+}
+static DwKernel dw_kernel(int N) {
+  switch (N) {
+#define DGM_CASE(n) \
+  case n: return dw_gemm_kernel<n>;
+    DGM_GEMM_NS(DGM_CASE)
+#undef DGM_CASE
+  }
+  return nullptr;
 }
 
 cudaError_t launch_layer_gemm(const LayerArgs& g, cudaStream_t s) {
   static unsigned long long attr = 0;  // per device
   if (once_per_device(attr)) {
-    cudaFuncSetAttribute(layer_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, LG_SMEM);
-    cudaFuncSetAttribute(layer_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, LGR_SMEM);
+    for (int n = 16; n <= 256; n += 16) {
+      cudaFuncSetAttribute(layer_kernel(false, n), cudaFuncAttributeMaxDynamicSharedMemorySize, LG_SMEM);
+      cudaFuncSetAttribute(layer_kernel(true, n), cudaFuncAttributeMaxDynamicSharedMemorySize, LGR_SMEM);
+    }
   }
   if (g.tiles <= 0) return cudaSuccess;
+  if (g.N % 16 != 0 || g.N < 16 || g.N > 256 || g.K % 16 != 0 || g.K <= 0) return cudaErrorInvalidValue;
   // split-precision layers whose weights fit 128 KB keep B_hi in shared memory for the CTA's lifetime (every
   // 256-wide layer; the K = 320 skip layer streams).  Single-pass launches (the backward, bf16 mode) stay on the
-  // streaming variant: measured, residency gains them nothing at 100k-200k points and costs a serialised 128 KB
-  // prologue per CTA at 10k.  DGMESH_B200_MLP_STREAM=1 forces the streaming variant everywhere (A/B comparison).
+  // streaming variant.  DGMESH_B200_MLP_STREAM=1 forces the streaming variant everywhere (A/B comparison).
   static const bool force_stream = [] {
     const char* e = getenv("DGMESH_B200_MLP_STREAM");
     return e && e[0] == '1';
   }();
   const bool resident = !force_stream && g.A_lo != nullptr && (size_t)(g.K >> 3) * g.N * 16 <= LGR_B_BYTES;
-  if (resident) layer_gemm_kernel<true><<<min(g.tiles, sm_count()), LG_THREADS, LGR_SMEM, s>>>(g);
-  else layer_gemm_kernel<false><<<min(g.tiles, sm_count()), LG_THREADS, LG_SMEM, s>>>(g);
+  layer_kernel(resident, g.N)<<<min(g.tiles, sm_count()), GEMM_THREADS, resident ? LGR_SMEM : LG_SMEM, s>>>(g);
   return cudaGetLastError();
 }
 
 // X has 256 features (two 128-feature halves -> grid.y = 2)
 cudaError_t launch_dw_gemm(const DwArgs& g, cudaStream_t s) {
   static unsigned long long attr = 0;  // per device
-  if (once_per_device(attr)) cudaFuncSetAttribute(dw_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DW_SMEM);
+  if (once_per_device(attr))
+    for (int n = 16; n <= 256; n += 16)
+      cudaFuncSetAttribute(dw_kernel(n), cudaFuncAttributeMaxDynamicSharedMemorySize, DW_SMEM);
   if (g.tiles <= 0) return cudaSuccess;
+  if (g.N % 16 != 0 || g.N < 16 || g.N > 256) return cudaErrorInvalidValue;
   dim3 grid(min(g.tiles, max(1, sm_count() / 2)), 2);
-  dw_gemm_kernel<<<grid, DW_THREADS, DW_SMEM, s>>>(g);
+  dw_kernel(g.N)<<<grid, GEMM_THREADS, DW_SMEM, s>>>(g);
   return cudaGetLastError();
 }
 
@@ -468,7 +493,7 @@ cudaError_t launch_mlp_backward(const DglNet& n, int P, const float* x, const fl
     // per-row feature gradients, or (uniform time, flag on the device) their column sums in row 0 of tile 0
     cudaMemsetAsync(b.tsum, 0, 32 * sizeof(float), s);
     tfeat_grad_kernel<<<(Pp + 255) / 256, 256, 0, s>>>(Pp, n.in_t, b.tu, b.dE, b.dZt1);
-    tfeat_colsum_kernel<<<min(592, (Pp + 7) / 8), 256, 0, s>>>(Pp, n.in_t, b.tu, b.dE, b.tsum);
+    tfeat_colsum_kernel<<<min(4 * sm_count(), (Pp + 7) / 8), 256, 0, s>>>(Pp, n.in_t, b.tu, b.dE, b.tsum);
     tfeat_row0_kernel<<<1, ACT_R, 0, s>>>(b.tu, b.tsum, b.dZt1);
     const int* td = b.tu + 1;
     CK(dw(vT1, vZt1, 32, tiles, gr.dWt1, WID, 1, s, nullptr, gr.dbt1, td));  // dWt1[32,256] = dZt1^T . T1 (transposed form)

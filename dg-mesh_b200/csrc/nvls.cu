@@ -2,8 +2,7 @@
 //
 // The one collective of the path is an all-reduce (sum) of ONE flat fp32 gradient buffer
 // [canonical-Gaussian gradients || MLP gradients] (23.6 MB at C2, 60 MB at C4).  At these sizes NCCL's
-// all-reduce is latency-bound (measured 0.12 ms for 23.6 MB on 8 B200s = 340 GB/s bus bandwidth, a fifth of
-// what the switch moves).  With the buffer in symmetric memory mapped through an NVSwitch MULTICAST object,
+// all-reduce is latency-bound.  With the buffer in symmetric memory mapped through an NVSwitch MULTICAST object,
 // the reduction is done by the switch itself:
 //     rank r owns slice r of the buffer:  v = multimem.ld_reduce.add(slice r)    -- the switch fetches the N
 //                                                                                   replicas, adds them, returns one

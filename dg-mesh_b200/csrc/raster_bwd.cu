@@ -1,4 +1,4 @@
-// raster_bwd.cu -- backward pass of the tile-based 3D-Gaussian rasterizer for sm_100a.
+// raster_bwd.cu -- backward pass of the tile-based 3D-Gaussian rasterizer for sm_90a.
 //
 //   render_bwd_kernel      gradient of the alpha-composite (role of renderCUDA,
 //                          dgr/cuda_rasterizer/backward.cu:399-557)
@@ -176,7 +176,7 @@ __global__ void __launch_bounds__(256, 4) render_bwd_kernel(
       }
       keep[k] = __ballot_sync(0xffffffffu, kp);
     }
-    // ---- back to front, two records per iteration (packed fp32x2 quadratic form, one
+    // ---- back to front, two records per iteration (two-lane quadratic form, one
     // butterfly reduction for both).  A is the record nearer the back (processed first).
     // Per lane only MOMENTS of w = G * dL/dG are accumulated (w, w dx, w dy, w dx^2, w dx dy,
     // w dy^2) plus the colour weights; the per-Gaussian factors (conic, opacity, viewport
@@ -194,15 +194,15 @@ __global__ void __launch_bounds__(256, 4) render_bwd_kernel(
         const int jA = k * 32 + bA, jB = k * 32 + bB;
         const float4 geA = s_geo[st][jA], geB = s_geo[st][jB];
         const float4 coA = s_attr[st][2 * jA], coB = s_attr[st][2 * jB];
-        const float2 dx2 = __fadd2_rn(make_float2(geA.x, geB.x), npx2);
-        const float2 dy2 = __fadd2_rn(make_float2(geA.y, geB.y), npy2);
-        float2 m1 = __fmul2_rn(dy2, make_float2(coA.z, coB.z));
-        const float2 m2 = __fmul2_rn(dx2, make_float2(coA.x, coB.x));
-        m1 = __fmul2_rn(dy2, m1);
-        const float2 sq = __ffma2_rn(dx2, m2, m1);
-        float2 m3 = __fmul2_rn(dx2, make_float2(coA.y, coB.y));
-        m3 = __fmul2_rn(dy2, m3);
-        const float2 npow = __ffma2_rn(sq, make_float2(0.5f, 0.5f), m3);  // = -power
+        const float2 dx2 = add2_rn(make_float2(geA.x, geB.x), npx2);
+        const float2 dy2 = add2_rn(make_float2(geA.y, geB.y), npy2);
+        float2 m1 = mul2_rn(dy2, make_float2(coA.z, coB.z));
+        const float2 m2 = mul2_rn(dx2, make_float2(coA.x, coB.x));
+        m1 = mul2_rn(dy2, m1);
+        const float2 sq = fma2_rn(dx2, m2, m1);
+        float2 m3 = mul2_rn(dx2, make_float2(coA.y, coB.y));
+        m3 = mul2_rn(dy2, m3);
+        const float2 npow = fma2_rn(sq, make_float2(0.5f, 0.5f), m3);  // = -power
         // order-dependent part (scalar): transmittance and the colour behind each record
         float wq[2], atq[2];
         bool contrib = false;
@@ -242,10 +242,10 @@ __global__ void __launch_bounds__(256, 4) render_bwd_kernel(
           const float2 at2 = up ? make_float2(atq[1], atq[0]) : make_float2(atq[0], atq[1]);
           const float2 ex2 = up ? make_float2(dx2.y, dx2.x) : dx2;
           const float2 ey2 = up ? make_float2(dy2.y, dy2.x) : dy2;
-          const float2 wx = __fmul2_rn(w2, ex2), wy = __fmul2_rn(w2, ey2);
-          const float2 wxx = __fmul2_rn(wx, ex2), wxy = __fmul2_rn(wx, ey2), wyy = __fmul2_rn(wy, ey2);
-          const float2 c0 = __fmul2_rn(at2, make_float2(dLp0, dLp0)), c1 = __fmul2_rn(at2, make_float2(dLp1, dLp1)),
-                       c2 = __fmul2_rn(at2, make_float2(dLp2, dLp2));
+          const float2 wx = mul2_rn(w2, ex2), wy = mul2_rn(w2, ey2);
+          const float2 wxx = mul2_rn(wx, ex2), wxy = mul2_rn(wx, ey2), wyy = mul2_rn(wy, ey2);
+          const float2 c0 = mul2_rn(at2, make_float2(dLp0, dLp0)), c1 = mul2_rn(at2, make_float2(dLp1, dLp1)),
+                       c2 = mul2_rn(at2, make_float2(dLp2, dLp2));
           v[0][0] = w2.x, v[1][0] = w2.y;
           v[0][1] = wx.x, v[1][1] = wx.y;
           v[0][2] = wy.x, v[1][2] = wy.y;

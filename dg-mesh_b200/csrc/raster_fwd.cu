@@ -1,4 +1,4 @@
-// raster_fwd.cu -- forward pass of the tile-based 3D-Gaussian rasterizer for sm_100a.
+// raster_fwd.cu -- forward pass of the tile-based 3D-Gaussian rasterizer for sm_90a.
 //
 // Pipeline (one stream, no host synchronisation):
 //   memset(tile counters) -> preprocess_kernel -> tile_scan_kernel -> scatter_kernel
@@ -690,10 +690,10 @@ __global__ void __launch_bounds__(256, 5) render_fwd_kernel(const uint2* __restr
     if (lane == 0) atomicAdd(&g_dbg_pairs[2], (unsigned long long)nb);
 #endif
     // ---- blend the survivors front to back, two records per iteration: the quadratic
-    // form of both is evaluated with packed fp32x2 instructions (FADD2/FMUL2/FFMA2, new on
-    // sm_100), the order-dependent transmittance update stays scalar.  The operation
+    // forms of both are evaluated side by side (add2_rn / mul2_rn / fma2_rn), the
+    // order-dependent transmittance update stays scalar.  The operation
     // sequence (which product is fused into which FMA) is the one nvcc emits for the
-    // reference's renderCUDA (forward.cu:330-352; see profiles/ref_render_fwd_sass.txt),
+    // reference's renderCUDA (forward.cu:330-352),
     // written with explicit-rounding intrinsics so it cannot be re-associated.
 #pragma unroll
     for (int k = 0; k < RB / 32; ++k) {
@@ -709,15 +709,15 @@ __global__ void __launch_bounds__(256, 5) render_fwd_kernel(const uint2* __restr
         const int jA = k * 32 + bA, jB = k * 32 + bB;
         const float4 geA = s_geo[st][jA], geB = s_geo[st][jB];
         const float4 coA = s_attr[st][2 * jA], coB = s_attr[st][2 * jB];
-        const float2 dx = __fadd2_rn(make_float2(geA.x, geB.x), npx2);
-        const float2 dy = __fadd2_rn(make_float2(geA.y, geB.y), npy2);
-        float2 m1 = __fmul2_rn(dy, make_float2(coA.z, coB.z));
-        const float2 m2 = __fmul2_rn(dx, make_float2(coA.x, coB.x));
-        m1 = __fmul2_rn(dy, m1);
-        const float2 sq = __ffma2_rn(dx, m2, m1);
-        float2 m3 = __fmul2_rn(dx, make_float2(coA.y, coB.y));
-        m3 = __fmul2_rn(dy, m3);
-        const float2 npow = __ffma2_rn(sq, make_float2(0.5f, 0.5f), m3);  // = -power (exactly)
+        const float2 dx = add2_rn(make_float2(geA.x, geB.x), npx2);
+        const float2 dy = add2_rn(make_float2(geA.y, geB.y), npy2);
+        float2 m1 = mul2_rn(dy, make_float2(coA.z, coB.z));
+        const float2 m2 = mul2_rn(dx, make_float2(coA.x, coB.x));
+        m1 = mul2_rn(dy, m1);
+        const float2 sq = fma2_rn(dx, m2, m1);
+        float2 m3 = mul2_rn(dx, make_float2(coA.y, coB.y));
+        m3 = mul2_rn(dy, m3);
+        const float2 npow = fma2_rn(sq, make_float2(0.5f, 0.5f), m3);  // = -power (exactly)
 #ifdef DGM_COUNT_PAIRS
         const uint32_t lc_before = last_contributor;
 #endif

@@ -20,6 +20,18 @@ __device__ const float kSH3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.4
                                   0.3731763325901154f,  -0.4570457994644658f, 1.445305721320277f,
                                   -0.5900435899266435f};
 
+// two-lane fp32 arithmetic with explicit rounding (one rounded operation per lane; Hopper has no
+// packed fp32x2 instructions, so each lane is a scalar FADD / FMUL / FFMA that cannot be re-associated)
+__device__ __forceinline__ float2 add2_rn(float2 a, float2 b) {
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
+}
+__device__ __forceinline__ float2 mul2_rn(float2 a, float2 b) {
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
+}
+__device__ __forceinline__ float2 fma2_rn(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+
 struct Mat3 {  // column-major like glm: c[col][row]
   float c[3][3];
 };

@@ -32,7 +32,7 @@ def densify_and_prune(self, max_grad, min_opacity, extent, max_screen_size):
     lib = _dgm_lib.lib()
     xyz = self._xyz
     if not xyz.is_cuda:
-        raise ValueError("densify_and_prune (B200): CUDA tensors required (no CPU fallback)")
+        raise ValueError("densify_and_prune : CUDA tensors required (no CPU fallback)")
     P, dev = xyz.shape[0], xyz.device
     if P == 0:
         return

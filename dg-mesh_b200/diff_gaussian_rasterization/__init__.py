@@ -1,4 +1,4 @@
-"""Drop-in `diff_gaussian_rasterization` backed by libdgmesh_b200.so (sm_100a).
+"""Drop-in `diff_gaussian_rasterization` backed by libdgmesh_b200.so (sm_90a).
 
 Mirrors the reference Python surface
 (dgmesh/submodules/diff-gaussian-rasterization/diff_gaussian_rasterization/__init__.py):

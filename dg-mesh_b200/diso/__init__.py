@@ -4,7 +4,7 @@
 
 `diso` is not vendored with the reference and cannot be installed offline, so this follows the
 CONTRACT visible at those call sites -- grid [G,G,G] fp32 -> (verts [V,3] fp32 in [0,1]^3, faces
-[F,3] integer), differentiable w.r.t. the grid -- with our own sm_100a marching cubes.  Vertex and
+[F,3] integer), differentiable w.r.t. the grid -- with our own sm_90a marching cubes.  Vertex and
 face ORDER are this implementation's (parity with diso is unpinned; see DESIGN.md)."""
 import os
 import sys
@@ -100,11 +100,11 @@ class DiffMC(nn.Module):
     def __init__(self, dtype=torch.float32):
         super().__init__()
         if dtype != torch.float32:
-            raise NotImplementedError("DiffMC (B200): float32 only (what DG-Mesh instantiates)")
+            raise NotImplementedError("DiffMC : float32 only (what DG-Mesh instantiates)")
 
     def forward(self, grid, deform=None, isovalue=0.0, normalize=True):
         if deform is not None:
-            raise NotImplementedError("DiffMC (B200): deform=None only (what DG-Mesh passes)")
+            raise NotImplementedError("DiffMC : deform=None only (what DG-Mesh passes)")
         verts, faces = _MCFunction.apply(grid, float(isovalue), bool(normalize))
         return verts, faces.long()
 

@@ -3,7 +3,7 @@ is single-process (dgmesh/train.py renders one frame per iteration on cuda:0).
 
 A frame's forward/backward depends only on the replicated parameters, its camera and its time, so
 frame k of a batch goes to rank k % world and the only data-path exchange is ONE all-reduce (NCCL over
-NVLink on the B200 box, gloo in the CPU tests) of a single flat fp32 buffer holding every gradient:
+NVLink on a multi-GPU H100 node, gloo in the CPU tests) of a single flat fp32 buffer holding every gradient:
 canonical-Gaussian parameters followed by the MLP parameters.  Batch of one frame per step -> no
 collective at all.  Densification statistics need the same reduction so all ranks prune identically
 (gaussian_model_dpsr_dynamic_anchor.py:679-682)."""
@@ -19,7 +19,7 @@ if _root not in sys.path:
 
 
 def shard_frames(n_frames, rank, world):
-    """Frame indices of this rank (round-robin, like the one-frame-per-GPU layout of the 8xB200 box)."""
+    """Frame indices of this rank (round-robin, like the one-frame-per-GPU layout of an 8-GPU node)."""
     return [k for k in range(n_frames) if k % world == rank]
 
 
@@ -98,7 +98,7 @@ class NvlsFlatGrad(FlatGrad):
     no multicast support (use `FlatGrad` there).  torch's symmetric-memory allocator is plumbing: it provides
     the memory, the multicast address and the signal pads; the collective itself is ours."""
 
-    BLOCKS = 296     # two per SM: enough multimem requests in flight to fill the links
+    BLOCKS = 264     # two per SM (H100: 132): enough multimem requests in flight to fill the links
     PAD_SKIP = 128
 
     def __init__(self, params, group=None):

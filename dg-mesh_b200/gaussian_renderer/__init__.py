@@ -3,7 +3,7 @@
 `render(viewpoint_camera, pc, pipe, bg_color, d_xyz, d_rotation, d_scaling, is_6dof=False,
 scaling_modifier=1.0, override_color=None)` keeps its signature and its four-key result dict
 ("render", "viewspace_points", "visibility_filter", "radii"); the rasterizer underneath is the
-sm_100a one (diff_gaussian_rasterization in this package).  `render_batch` is the multi-frame
+sm_90a one (diff_gaussian_rasterization in this package).  `render_batch` is the multi-frame
 variant used for data-parallel training over frames (one call, one gradient accumulation)."""
 import math
 

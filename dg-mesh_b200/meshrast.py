@@ -1,4 +1,4 @@
-"""Differentiable triangle-mesh rasterisation on the B200 (SURVEY.md 8(f)-1), with the call surface of the
+"""Differentiable triangle-mesh rasterisation on the GPU (SURVEY.md 8(f)-1), with the call surface of the
 three nvdiffrast primitives dgmesh/utils/renderer.py:33-121 uses, so that render_mask / render_mesh read
 exactly like the reference:
 

@@ -1,4 +1,4 @@
-"""Drop-in `nvdiffrast_utils.dpsr.DPSR` backed by libdgmesh_b200.so (sm_100a kernels + cuFFT).
+"""Drop-in `nvdiffrast_utils.dpsr.DPSR` backed by libdgmesh_b200.so (sm_90a kernels + cuFFT).
 
 Mirrors dgmesh/nvdiffrast_utils/dpsr.py:10-70:
     DPSR(res, sig=10, scale=True, shift=True);  forward(V[b,nv,3], N[b,nv,3]) -> phi[b,*res]
@@ -71,16 +71,16 @@ class DPSR(nn.Module):
     def __init__(self, res, sig=10, scale=True, shift=True):
         super().__init__()
         if len(res) != 3 or not (res[0] == res[1] == res[2]) or res[0] % 2:
-            raise NotImplementedError("DPSR (B200): cubic 3-D grids with an even resolution only")
+            raise NotImplementedError("DPSR : cubic 3-D grids with an even resolution only")
         if not (scale and shift):
-            raise NotImplementedError("DPSR (B200): scale=True, shift=True only (DG-Mesh's configuration)")
+            raise NotImplementedError("DPSR : scale=True, shift=True only (DG-Mesh's configuration)")
         self.res, self.sig, self.dim = tuple(res), sig, 3
         self.scale, self.shift = scale, shift
 
     def _check(self, V, N):
         assert V.shape == N.shape  # dpsr.py:34
         if V.dim() != 3 or V.shape[0] != 1:
-            raise NotImplementedError("DPSR (B200): batch size 1 only")
+            raise NotImplementedError("DPSR : batch size 1 only")
 
     def forward(self, V, N):
         """phi [1, G, G, G] exactly as the reference returns it."""

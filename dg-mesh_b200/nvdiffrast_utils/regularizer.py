@@ -20,7 +20,7 @@ class _Laplacian(torch.autograd.Function):
     @staticmethod
     def forward(ctx, v_pos, tri):
         if not v_pos.is_cuda:
-            raise ValueError("laplace_regularizer_const (B200): CUDA tensors required (no CPU fallback)")
+            raise ValueError("laplace_regularizer_const : CUDA tensors required (no CPU fallback)")
         v = v_pos.contiguous().float()
         t = tri.to(torch.int32).contiguous()
         V, F = v.shape[0], t.shape[0]

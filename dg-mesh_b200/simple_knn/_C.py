@@ -1,4 +1,4 @@
-"""`simple_knn._C.distCUDA2` backed by libdgmesh_b200.so (sm_100a).
+"""`simple_knn._C.distCUDA2` backed by libdgmesh_b200.so (sm_90a).
 
 Mirrors dgmesh/submodules/simple-knn/spatial.cu:15-26 / ext.cpp:15-17:
     distCUDA2(points: cuda float32 [P,3]) -> cuda float32 [P]

@@ -37,7 +37,7 @@ class _ImageLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, img, gt, lam, mode):
         if not img.is_cuda or not gt.is_cuda:
-            raise ValueError("loss_utils (B200): CUDA tensors required (no CPU fallback)")
+            raise ValueError("loss_utils : CUDA tensors required (no CPU fallback)")
         if img.dim() != 3 or img.shape[0] != 3 or img.shape != gt.shape:
             raise ValueError("expected img and gt of shape [3, H, W]")
         x, y = img.detach().contiguous().float(), gt.detach().contiguous().float()
@@ -75,5 +75,5 @@ def image_loss(image, gt_image, lambda_dssim=0.2, return_parts=False):
 def ssim(img1, img2, window_size=11, size_average=True):
     """Mean SSIM of two [3,H,W] images (loss_utils.py:39-76: window 11, sigma 1.5)."""
     if window_size != 11 or not size_average:
-        raise NotImplementedError("loss_utils (B200): window_size=11, size_average=True (what train.py uses) only")
+        raise NotImplementedError("loss_utils : window_size=11, size_average=True (what train.py uses) only")
     return _ImageLoss.apply(img1, img2, 1.0, 1)[0]

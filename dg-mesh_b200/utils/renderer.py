@@ -2,7 +2,7 @@
 marching cubes -> per-vertex colour -> mesh rasterisation (mask + image), i.e. the whole mesh branch of the
 training step.  Same signatures, same return values.
 
-What changes underneath: DPSR and marching cubes are the sm_100a kernels of this package; when
+What changes underneath: DPSR and marching cubes are the sm_90a kernels of this package; when
 `gaussians.dpsr` is this package's DPSR, the sign fix + threshold that follow the solve (reference
 :163-168) are fused into it, which removes the host read of psr[0,0,0,0].  The mesh RASTERISATION
 (`render_mask` / `render_mesh`, reference :33-121: nvdiffrast's rasterize / interpolate / antialias on an

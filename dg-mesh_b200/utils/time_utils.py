@@ -1,13 +1,13 @@
 """Drop-in `utils.time_utils` (reference: dgmesh/utils/time_utils.py): DeformNetwork,
 DeformNetworkNormal, DeformNetworkNormalSep, AppearanceNetwork with the SAME constructor
 signatures, parameter names / shapes (state_dicts are interchangeable) and return values, but the
-forward + backward run as bf16 tcgen05 GEMM chains inside libdgmesh_b200.so.
+forward + backward run as bf16 wgmma GEMM chains inside libdgmesh_b200.so.
 
 `utils` is a namespace package in the reference (no __init__.py) and here: with this directory
 ahead of the reference's on sys.path only `utils.time_utils` is replaced.
 
 Numerics (the reference is fp32 cuBLAS).  Default `DGMESH_B200_MLP_PRECISION=bf16x3`: the forward
-runs every layer as three bf16 tcgen05 passes over split operands (hi + lo, fp32 accumulation), so
+runs every layer as three bf16 wgmma passes over split operands (hi + lo, fp32 accumulation), so
 outputs agree with the fp32 reference to ~1e-5 and the ReLU decisions are the reference's; the
 backward is single-pass bf16 and the parameter / input gradients agree to <= 2 % relative L2
 (measured 0.3-1 %).  `bf16`: single-pass forward, 3x fewer MMAs; outputs ~2e-3, but ~1 % of the
@@ -76,7 +76,7 @@ class _MLPFunction(torch.autograd.Function):
     def forward(ctx, spec, train, x, t, *params):
         lib = _dgm_lib.lib()
         if not x.is_cuda:
-            raise ValueError("time_utils (B200): CUDA tensors required (no CPU fallback)")
+            raise ValueError("time_utils : CUDA tensors required (no CPU fallback)")
         xc = x.detach().contiguous().float()
         tc = t.detach().contiguous().float().reshape(-1)
         P = xc.shape[0]
@@ -147,7 +147,7 @@ class _TimeNet(nn.Module):
     def __init__(self, D=8, W=256, input_ch=3, output_ch=59, multires=10, is_blender=False, is_6dof=False):
         super().__init__()
         if D != 8 or W != 256 or multires != 10:
-            raise NotImplementedError("time_utils (B200): D=8, W=256, multires=10 (the reference defaults) only")
+            raise NotImplementedError("time_utils : D=8, W=256, multires=10 (the reference defaults) only")
         self.D, self.W, self.input_ch, self.output_ch = D, W, input_ch, output_ch
         self.t_multires = 6 if is_blender else 10
         self.skips = [D // 2]

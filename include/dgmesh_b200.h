@@ -1,5 +1,5 @@
 /*
- * dgmesh_b200.h -- C-ABI of the B200-native DG-Mesh hot path (libdgmesh_b200.so).
+ * dgmesh_b200.h -- C-ABI of the H100-native DG-Mesh hot path (libdgmesh_b200.so).
  *
  * Drop-in boundary: every entry point below stands in for one native interface
  * of the reference (Isabella98Liu/DG-Mesh @ 754f42c); the reference file:line it
@@ -33,7 +33,7 @@ extern "C" {
 #define DGM_E_WORKSPACE (-2) /* a workspace is smaller than the query says */
 #define DGM_E_LAUNCH (-3)    /* cudaGetLastError() != cudaSuccess after enqueue */
 
-/* library / build identification ("dgmesh_b200 <ver> sm_100a") */
+/* library / build identification ("dgmesh_b200 <ver> sm_90a") */
 const char* dgm_version(void);
 /* cudaGetErrorString of the last launch error seen by this thread (or "") */
 const char* dgm_last_error(void);
@@ -277,8 +277,8 @@ int dgmc_backward(int G, int V, const float* phi, float iso, void* ws, size_t ws
                   const float* dL_dverts, float* dL_dphi, void* stream);
 
 /* ------------------------------------------------------------------------
- * Tensor-core GEMM building blocks of the MLPs (tcgen05.mma, bf16 operands, fp32 accumulation in
- * TMEM), exposed stand-alone for the parity tests (torch.matmul on the same bf16 operands is the
+ * Tensor-core GEMM building blocks of the MLPs (wgmma, bf16 operands, fp32 accumulation in
+ * registers), exposed stand-alone for the parity tests (torch.matmul on the same bf16 operands is the
  * oracle).  The networks below drive the same two kernels on activations kept in the library's
  * blocked layout; these entry points first copy the row-major operands into that layout inside
  * `ws` (dgl_gemm_ws_bytes(M, N, K), with M = the long dimension).
@@ -298,7 +298,7 @@ int dgl_gemm_tn_bf16(int P, int Mf, int Nf, const void* X, int ldx, const void* 
  * DeformNetworkNormal, DeformNetworkNormalSep, AppearanceNetwork; driven through
  * DeformModel*.step / AppearanceModel.step, dgmesh/scene/deform_model.py, appearance_model.py).
  * The reference runs ~30 fp32 cuBLAS / elementwise kernels per call; here the whole network is a
- * chain of bf16 tcgen05 GEMMs (fp32 accumulation) with fused bias / ReLU epilogues.
+ * chain of bf16 wgmma GEMMs (fp32 accumulation) with fused bias / ReLU epilogues.
  *
  * DglNet describes one network with PACKED parameters (built by dgl_mlp_pack): bf16 weights in the
  * blocked operand layout of the GEMM kernels (dg-mesh_b200/csrc/mlp_gemm.cuh: element (row, k) of
@@ -330,7 +330,7 @@ typedef struct DglNet {
   const float* bt1;  /* [32] */
   /* Forward precision.  precise != 0 ("bf16x3", what dgl_mlp_pack sets): every forward operand is a
    * PAIR of bf16 numbers hi + lo (lo = rounding residual) and each layer accumulates
-   * A_hi B_hi + A_lo B_hi + A_hi B_lo in fp32 -- three tcgen05 passes into one TMEM accumulator, ~16
+   * A_hi B_hi + A_lo B_hi + A_hi B_lo in fp32 -- three wgmma passes into one accumulator, ~16
    * mantissa bits per operand, so activations and ReLU decisions match the reference's fp32 cuBLAS
    * to ~1e-5 (a single bf16 pass differs by ~2e-3, enough to flip ReLU signs and move the gradients
    * by ~7 %, see DESIGN.md).  precise == 0: single bf16 pass (3x fewer MMAs).  The backward pass is

@@ -22,7 +22,7 @@ and, as the equivalent of `pip install --target` (build OUTPUT, git-ignored):
   oracle/_ref/dgmesh/        the reference's whole Python tree minus submodules/ (train.py, scene/,
         utils/, arguments/, configs/): what tools/train_harness.py runs UNMODIFIED
 
-The reference ships no sm_100 build; it needs two forced includes under gcc 13
+The reference ships no sm_90a build; it needs two forced includes under gcc 13
 (`<cstdint>` for rasterizer_impl.h, `<cfloat>` for simple_knn.cu) -- passed on
 the command line, the sources are not patched.  We use torch's own JIT
 extension builder (ninja + nvcc), not the reference's setup.py / CMake.
@@ -48,7 +48,7 @@ def _load(name, sources, build_dir, extra_cuda, extra_inc):
         extra_include_paths=extra_inc,
         extra_cflags=["-O3", "-include", "cstdint", "-include", "cfloat"],
         extra_cuda_cflags=["-O3", "-include", "cstdint", "-include", "cfloat",
-                           "-gencode", "arch=compute_100,code=sm_100"] + extra_cuda,
+                           "-gencode", "arch=compute_90a,code=sm_90a"] + extra_cuda,
         build_directory=build_dir,
         with_cuda=True,
         is_python_module=False,   # do not import here (no GPU needed, but keep it lazy)

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Generate golden input/output vectors by running the UNMODIFIED reference rasterizer
-(oracle/_ref, built from /root/reference by oracle/build_ref.py) on the B200 box:
+(oracle/_ref, built from /root/reference by oracle/build_ref.py) on a GPU:
 
     gpurun -- 'python tests/golden/make_golden.py gpurun_out/golden'   # then copy *.npz to tests/golden/
 

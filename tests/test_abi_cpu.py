@@ -28,7 +28,7 @@ def test_binding_covers_header(repo_root):
     import _dgm_lib
     assert sorted(_dgm_lib.SIGNATURES) == _declared(repo_root)
     lib = _dgm_lib.lib()
-    assert b"sm_100a" in lib.dgm_version()
+    assert b"sm_90a" in lib.dgm_version()
 
 
 def test_workspace_query_and_argument_errors():

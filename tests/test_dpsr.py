@@ -1,5 +1,8 @@
 """DPSR parity: numpy oracle vs the reference's own PyTorch code (CPU, pins the oracle), and the
-CUDA path vs the reference (forward and autograd gradients) on the GPU."""
+CUDA path vs the reference (forward and autograd gradients) on the GPU.  Where oracle/_ref is not built the
+reference is its restatement tests/ref_dpsr.py, pinned here to the reference's stored outputs."""
+import os
+
 import numpy as np
 import pytest
 import torch
@@ -31,11 +34,22 @@ def affine_close(a, b, resid_tol=5e-5, scale_tol=5e-3):
     return abs(alpha - 1) < scale_tol and resid < resid_tol, (alpha, beta, resid)
 
 
-ref = util.load_reference_pymodules()
-needs_ref = pytest.mark.skipif(ref is None, reason="oracle/_ref/refpy missing (run oracle/build_ref.py)")
+ref = util.load_reference_dpsr()
 
 
-@needs_ref
+def test_dpsr_restatement_matches_reference_golden_cpu():
+    """tests/ref_dpsr.py (the reference's DPSR where oracle/_ref is not built) reproduces the reference's stored
+    field and autograd gradients."""
+    import ref_dpsr
+    z = np.load(os.path.join(os.path.dirname(__file__), "golden", "dpsr_g32.npz"))
+    V = torch.from_numpy(z["V"]).requires_grad_(True)
+    N = torch.from_numpy(z["N"]).requires_grad_(True)
+    phi = ref_dpsr.DPSR(res=(32, 32, 32), sig=float(z["sig"]))(V[None], N[None])[0]
+    (phi * torch.from_numpy(z["gout"])).sum().backward()
+    assert util.rel_err(phi.detach(), z["phi"]) < 1e-5
+    assert util.rel_err(V.grad, z["dV"]) < 1e-5 and util.rel_err(N.grad, z["dN"]) < 1e-5
+
+
 @pytest.mark.parametrize("G,n,sig", [(16, 300, 2.0), (32, 2000, 3.0)])
 def test_oracle_matches_reference_dpsr_cpu(G, n, sig):
     V, N = _points(n, G)
@@ -46,7 +60,6 @@ def test_oracle_matches_reference_dpsr_cpu(G, n, sig):
 
 
 @pytest.mark.gpu
-@needs_ref
 @pytest.mark.parametrize("G,n,sig", [(32, 3000, 3.0), (64, 20000, 3.0), (288, 200_000, 3.0)])
 def test_cuda_dpsr_matches_reference(G, n, sig):
     from nvdiffrast_utils.dpsr import DPSR
@@ -70,7 +83,6 @@ def test_cuda_dpsr_matches_reference(G, n, sig):
 
 
 @pytest.mark.gpu
-@needs_ref
 def test_cuda_dpsr_signed_variant_matches_mesh_renderer_glue():
     """forward_signed == psr * sign - thres as utils/renderer.py:163-168 computes it (values + grads)."""
     from nvdiffrast_utils.dpsr import DPSR

@@ -45,6 +45,27 @@ def test_dropin_modules_initialise_like_the_reference_and_restatement_matches_cp
     assert util.rel_err(y, z["y"]) < 3e-2          # bf16 operands vs the fp32 reference
 
 
+@pytest.mark.parametrize("path", MLP_FILES, ids=[os.path.basename(f) for f in MLP_FILES])
+def test_fp32_network_restatement_matches_reference_golden_cpu(path):
+    """tests/ref_time_utils.py (the reference networks where oracle/_ref is not built) reproduces the reference's
+    stored fp32 outputs and gradients."""
+    import ref_time_utils
+    z, mine, x, t, gout, _ = _mlp_case(path, "cpu")
+    cls = type(mine).__name__
+    net = getattr(ref_time_utils, cls)(is_blender=mine.is_blender)
+    net.load_state_dict(mine.state_dict())
+    xa = x.clone().requires_grad_(True)
+    out = net(xa, t)
+    y = torch.cat(out if isinstance(out, tuple) else (out,), -1)
+    assert util.rel_l2(y, z["y"]) < 1e-5 and util.rel_err(y, z["y"]) < 1e-4
+    (y * gout[:, :y.shape[1]]).sum().backward()
+    assert util.rel_l2(xa.grad, z["dx"]) < 1e-4
+    for k, p in net.named_parameters():
+        key = "g_" + k.replace(".", "__")
+        if key in z.files:
+            assert util.rel_l2(p.grad, z[key]) < 1e-4, k
+
+
 def test_numpy_dpsr_oracle_matches_reference_golden_cpu():
     z = np.load(os.path.join(GOLD, "dpsr_g32.npz"))
     phi = dpsr_forward_np(z["V"], z["N"], 32, float(z["sig"]))

@@ -13,17 +13,19 @@ from oracle.oracle import image_loss_np
 
 
 def _ref_loss_utils():
-    for p in (os.path.join(util.REF_DIR, "refpy", "loss_utils.py"), "/root/reference/dgmesh/utils/loss_utils.py"):
-        if os.path.exists(p):
-            spec = importlib.util.spec_from_file_location("ref_loss_utils", p)
-            m = importlib.util.module_from_spec(spec)
-            spec.loader.exec_module(m)
-            return m
-    return None
+    """The reference's loss_utils where oracle/_ref is built, else its restatement tests/ref_loss_utils.py (pinned
+    to the numpy oracle by test_oracle_matches_reference_loss_and_autograd_cpu)."""
+    p = os.path.join(util.REF_DIR, "refpy", "loss_utils.py")
+    if os.path.exists(p):
+        spec = importlib.util.spec_from_file_location("ref_loss_utils_built", p)
+        m = importlib.util.module_from_spec(spec)
+        spec.loader.exec_module(m)
+        return m
+    import ref_loss_utils
+    return ref_loss_utils
 
 
 ref_lu = _ref_loss_utils()
-needs_ref = pytest.mark.skipif(ref_lu is None, reason="reference loss_utils.py not available")
 
 
 def _images(H, W, seed):
@@ -33,7 +35,6 @@ def _images(H, W, seed):
     return img, gt
 
 
-@needs_ref
 @pytest.mark.parametrize("H,W", [(40, 56), (33, 47), (8, 9)])
 def test_oracle_matches_reference_loss_and_autograd_cpu(H, W):
     img, gt = _images(H, W, H * W)
@@ -47,7 +48,6 @@ def test_oracle_matches_reference_loss_and_autograd_cpu(H, W):
 
 
 @pytest.mark.gpu
-@needs_ref
 @pytest.mark.parametrize("H,W", [(800, 800), (67, 45), (16, 16), (1080, 1920)])
 def test_cuda_image_loss_matches_reference(H, W):
     import importlib
@@ -93,21 +93,24 @@ def test_cuda_image_loss_against_numpy_oracle_and_errors():
 @pytest.mark.parametrize("sub", [2, 5])
 def test_cuda_laplacian_regulariser_matches_reference(sub):
     """nvdiffrast_utils.regularizer.laplace_regularizer_const (regularizer.py:40-59): fused forward / backward
-    against the reference's own function (imported unmodified from oracle/_ref/dgmesh) and its autograd."""
+    against the reference's own function (imported unmodified from oracle/_ref/dgmesh; where that is not built,
+    its restatement in tests/ref_loss_utils.py) and its autograd."""
     import importlib.util
     import os
     import sys
     ref_file = os.path.join(util.ROOT, "oracle", "_ref", "dgmesh", "nvdiffrast_utils", "regularizer.py")
-    if not os.path.exists(ref_file):
-        pytest.skip("oracle/_ref/dgmesh missing")
-    sys.path.insert(0, os.path.join(util.ROOT, "tools"))
-    import harness_stubs
-    harness_stubs.install()
-    import launch
-    launch.install(os.path.join(util.ROOT, "oracle", "_ref", "dgmesh"))
-    spec = importlib.util.spec_from_file_location("nvdiffrast_utils._ref_regularizer_for_test", ref_file)
-    refmod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(refmod)
+    built = os.path.exists(ref_file)
+    if built:
+        sys.path.insert(0, os.path.join(util.ROOT, "tools"))
+        import harness_stubs
+        harness_stubs.install()
+        import launch
+        launch.install(os.path.join(util.ROOT, "oracle", "_ref", "dgmesh"))
+        spec = importlib.util.spec_from_file_location("nvdiffrast_utils._ref_regularizer_for_test", ref_file)
+        refmod = importlib.util.module_from_spec(spec)
+        spec.loader.exec_module(refmod)
+    else:
+        import ref_loss_utils as refmod
     mine = importlib.import_module("nvdiffrast_utils.regularizer")
     assert mine.__file__.startswith(os.path.join(util.ROOT, "dg-mesh_b200"))
     from test_meshrast import icosphere
@@ -122,4 +125,5 @@ def test_cuda_laplacian_regulariser_matches_reference(sub):
     (la * 3.0).backward()
     (lb * 3.0).backward()
     assert util.rel_err(va.grad, vb.grad) < 1e-5
-    assert callable(mine.avg_edge_length)        # names this drop-in does not define fall through to the reference
+    if built:
+        assert callable(mine.avg_edge_length)    # names this drop-in does not define fall through to the reference

@@ -1,5 +1,5 @@
-"""Deformation / appearance MLPs: the tcgen05 GEMM chain vs (a) the reference's own fp32 PyTorch modules
-(oracle/_ref/refpy/time_utils.py) and (b) a bf16-rounding restatement of the reference network (same
+"""Deformation / appearance MLPs: the wgmma GEMM chain vs (a) the reference's own fp32 PyTorch modules
+(oracle/_ref/refpy/time_utils.py where built, else their fp32 restatement tests/ref_time_utils.py) and (b) a bf16-rounding restatement of the reference network (same
 rounding points as the single-pass kernels: bf16 operands, fp32 accumulate).
 
 Contract (DESIGN.md), relative L2 per tensor:
@@ -15,8 +15,7 @@ import torch
 
 import util
 
-ref = util.load_reference_pymodules()
-needs_ref = pytest.mark.skipif(ref is None, reason="oracle/_ref/refpy missing")
+ref = util.load_reference_networks()
 
 
 def bf(x):
@@ -69,7 +68,6 @@ def inputs(n, seed):
     return x, t
 
 
-@needs_ref
 def test_emulation_is_close_to_fp32_reference_cpu():
     torch.manual_seed(0)
     net = ref.time_utils.DeformNetworkNormal(is_blender=True)
@@ -80,7 +78,6 @@ def test_emulation_is_close_to_fp32_reference_cpu():
     assert util.rel_err(a, b) < 3e-2
 
 
-@needs_ref
 def test_single_pass_gap_is_forward_rounding_cpu():
     """Why the default is the split-precision forward: with bf16-rounded FORWARD operands alone (exact fp32
     backward) the gradients already differ from the fp32 reference by several per cent (ReLU sign flips),
@@ -106,7 +103,6 @@ def test_single_pass_gap_is_forward_rounding_cpu():
 
 
 @pytest.mark.gpu
-@needs_ref
 @pytest.mark.parametrize("prec", ["bf16x3", "bf16"])
 @pytest.mark.parametrize("cls,blender,n", [("DeformNetworkNormal", True, 3000), ("DeformNetworkNormal", False, 1000),
                                            ("DeformNetwork", True, 517), ("DeformNetworkNormalSep", True, 2048),

@@ -1,5 +1,5 @@
-"""The two tcgen05 GEMM kernels of the MLPs vs torch.matmul on the same bf16 operands (fp32 accumulate):
-`layer_gemm_kernel` (K-major operands, persistent, double-buffered TMEM) through dgl_gemm_bf16 and
+"""The two wgmma GEMM kernels of the MLPs vs torch.matmul on the same bf16 operands (fp32 accumulate):
+`layer_gemm_kernel` (K-major operands, persistent, register accumulators) through dgl_gemm_bf16 and
 `dw_gemm_kernel` (MN-major operands straight from the blocked activations) through dgl_gemm_tn_bf16."""
 import ctypes
 

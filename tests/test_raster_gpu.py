@@ -1,6 +1,8 @@
 """GPU parity tests of the rasterizer: the CUDA path through the C-ABI vs
-  (1) the UNMODIFIED reference extension (oracle/_ref, built from /root/reference),
-  (2) the CPU oracle (oracle/liboracle.so), and
+  (1) the UNMODIFIED reference extension (oracle/_ref, built by oracle/build_ref.py from the DG-Mesh sources)
+      where it has been built, else the CPU oracle in its place (oracle/liboracle.so, the C restatement of the
+      reference that tests/test_golden_cpu.py pins to the reference's own stored outputs),
+  (2) the CPU oracle directly, and
   (3) size-independent properties at the full benchmark size.
 Bar: integer state bit-exact (radii, tiles_touched, sorted keys, point list, ranges,
 n_contrib); image and all gradients within 1e-4 of the tensor's scale (fp32).
@@ -70,8 +72,54 @@ def run_ours(sc, cam, bg, degree=3, use_colors=False, use_cov=False, dpix=None, 
     return out
 
 
+def run_oracle(sc, cam, bg, degree=3, use_colors=False, use_cov=False, dpix=None, scale_modifier=1.0):
+    """run_ref's result computed by the CPU oracle: the same state arrays, dtypes and gradients."""
+    from oracle.oracle import RasterOracle
+    cpu = {k: v.detach().cpu() for k, v in sc.items()}
+    kw = dict(means3D=cpu["means3D"].numpy(), opacities=cpu["opacities"].numpy(),
+              view=cam.world_view_transform.cpu().numpy(), proj=cam.full_proj_transform.cpu().numpy(),
+              campos=cam.camera_center.cpu().numpy(), W=cam.image_width, H=cam.image_height,
+              tan_fovx=math.tan(cam.FoVx * 0.5), tan_fovy=math.tan(cam.FoVy * 0.5),
+              bg=bg.detach().cpu().numpy().astype(np.float32), scale_modifier=scale_modifier)
+    if use_colors:
+        kw["colors_precomp"] = cpu["shs"][:, 0, :].abs().numpy()
+    else:
+        kw["shs"], kw["degree"] = cpu["shs"].numpy(), degree
+    if use_cov:
+        kw["cov3D_precomp"] = util.cov3d_torch(cpu["scales"], cpu["rotations"]).numpy()
+    else:
+        kw["scales"], kw["rotations"] = cpu["scales"].numpy(), cpu["rotations"].numpy()
+    orc = RasterOracle(32)
+    o = orc.forward(**kw)
+    dev = sc["means3D"].device
+
+    def t(a, dtype=None):
+        a = torch.from_numpy(np.ascontiguousarray(a))
+        return (a.view(dtype) if dtype is not None else a).to(dev)
+    out = dict(color=t(o["color"]), radii=t(o["radii"]), R=int(o["num_rendered"]), depths=t(o["depths"]),
+               means2D=t(o["means2D"]), cov3D=t(o["cov3D"]), conic_opacity=t(o["conic_opacity"]), rgb=t(o["rgb"]),
+               tiles_touched=t(o["tiles_touched"], torch.int32), point_list_keys=t(o["point_list_keys"], torch.int64),
+               point_list=t(o["point_list"], torch.int32), ranges=t(o["ranges"], torch.int32),
+               final_T=t(o["final_T"]), n_contrib=t(o["n_contrib"], torch.int32))
+    if dpix is not None:
+        g = orc.backward(o, dpix.detach().cpu().numpy())
+        P = cpu["means3D"].shape[0]
+        grads = dict(means3D=t(g["dL_dmean3D"]), opacities=t(g["dL_dopacity"]).reshape(cpu["opacities"].shape),
+                     scales=None if use_cov else t(g["dL_dscale"]), rotations=None if use_cov else t(g["dL_drot"]),
+                     shs=None if use_colors else t(g["dL_dsh"]).reshape(cpu["shs"].shape),
+                     means2D=t(g["dL_dmean2D"]))
+        if use_colors:
+            grads["colors"] = t(g["dL_dcolor"]).reshape(P, 3)
+        if use_cov:
+            grads["cov"] = t(g["dL_dcov3D"]).reshape(P, 6)
+        out["grads"] = grads
+    return out
+
+
 def run_ref(sc, cam, bg, degree=3, use_colors=False, use_cov=False, dpix=None, scale_modifier=1.0):
     ref = util.load_reference_rasterizer()
+    if ref is None:
+        return run_oracle(sc, cam, bg, degree, use_colors, use_cov, dpix, scale_modifier)
     import synth
     rs = synth.raster_settings_for(cam, bg, sh_degree=degree, scale_modifier=scale_modifier,
                                    settings_cls=ref.GaussianRasterizationSettings)
@@ -138,11 +186,6 @@ def compare(ours, ref, tol=TOL, check_grads=True, label="", skip=(), n_contrib_s
             assert e < tol, f"{label} grad {k}: {e}"
 
 
-needs_ref = pytest.mark.skipif(util.load_reference_rasterizer() is None,
-                               reason="oracle/_ref not built (run oracle/build_ref.py where /root/reference exists)")
-
-
-@needs_ref
 @pytest.mark.parametrize("n,W,H,degree,colors,cov,scale", [
     (3000, 160, 96, 3, False, False, 0.03),
     (3000, 160, 96, 0, False, False, 0.03),
@@ -165,7 +208,6 @@ def test_bit_exact_against_reference(n, W, H, degree, colors, cov, scale):
     compare(a, b, label=f"n={n} {W}x{H} deg={degree}", skip=skip)
 
 
-@needs_ref
 def test_long_tile_list_global_sort_path():
     """More instances in one tile than one shared-memory sort stage holds (3072): several runs per tile."""
     n = 9000
@@ -180,7 +222,6 @@ def test_long_tile_list_global_sort_path():
     compare(a, b, label="long list")
 
 
-@needs_ref
 def test_object_shaped_scene_dense_tiles_all_sort_regimes():
     """What DG-Mesh actually trains on: an object filling a fraction of the image -- thousands of instances per tile
     inside a narrow depth range, i.e. depth buckets of hundreds to thousands of keys.  Exercises the register, the
@@ -207,7 +248,6 @@ def test_object_shaped_scene_dense_tiles_all_sort_regimes():
     assert dgr._Sizing.hint[(torch.cuda.current_device(), 160, 128)][3] == int(lens.max())
 
 
-@needs_ref
 def test_one_depth_plane_block_longer_than_the_sort_stage():
     """Thousands of Gaussians at (almost) ONE view depth on a few tiles: a single depth block longer than the 3072-key
     stage is sorted in place in global memory.  A few far-away Gaussians keep the frame's depth range wide."""
@@ -228,7 +268,14 @@ def test_one_depth_plane_block_longer_than_the_sort_stage():
     compare(a, b, label="one-depth plane")
 
 
-@needs_ref
+# The CPU oracle evaluates exp() with the host's libm, the reference's CUDA build (like this one) with the
+# device's: over the hundreds of blended records per pixel of the full-size scenes the transmittance drifts past
+# 1e-4, so these two compare with the reference build only.
+needs_ref_build = pytest.mark.skipif(util.load_reference_rasterizer() is None,
+                                     reason="oracle/_ref not built (oracle/build_ref.py)")
+
+
+@needs_ref_build
 def test_full_size_config_c2_against_reference():
     """BASELINE.json configs[1]: 100k Gaussians, 800x800, SH degree 3."""
     import synth
@@ -241,6 +288,7 @@ def test_full_size_config_c2_against_reference():
     compare(a, b, label="C2")
 
 
+@needs_ref_build
 def test_largest_config_c5_against_reference():
     """BASELINE.json configs[4] shape: 500k Gaussians, 1920x1080 (1080 is not a multiple of 16:
     ragged last tile row; 8 160 tiles), SH degree 3 -- integer state bit-exact, image / gradients 1e-4."""
@@ -332,9 +380,6 @@ def test_unmodified_loop_survives_growing_R_without_exception():
     later.  The forward is re-run transparently when the optimistic capacity was too small."""
     import diff_gaussian_rasterization as dgr
     import synth
-    ref = util.load_reference_rasterizer()
-    if ref is None:
-        pytest.skip("reference extension not built")
     sc, _ = util.small_scene(n=3000, W=128, H=96, seed=4, scale=0.12)
     sc = _cuda(sc)
     bg = torch.tensor([0.1, 0.2, 0.3], device="cuda")

@@ -130,11 +130,38 @@ def load_reference_pymodules():
     of the hot path are exercised.  Returns None when neither location exists."""
     if "refpy" in sys.modules:
         return sys.modules["refpy"]
-    import types
-    from unittest import mock
     refpy = os.path.join(REF_DIR, "refpy")
     if not os.path.isdir(refpy):
         return None
+    return _load_refpy(refpy)
+
+
+def load_reference_networks():
+    """The reference's `time_utils` / `rigid_utils` for the MLP parity tests: the reference's own modules where
+    oracle/_ref/refpy is built, else the fp32 restatement (tests/ref_time_utils.py, pinned to the reference's
+    stored outputs by tests/test_golden_py.py) with this package's rigid_utils."""
+    ref = load_reference_pymodules()
+    if ref is not None:
+        return ref
+    import types
+    import ref_time_utils
+    return types.SimpleNamespace(time_utils=ref_time_utils, rigid_utils=importlib.import_module("utils.rigid_utils"))
+
+
+def load_reference_dpsr():
+    """The reference's `dpsr` for the DPSR parity tests: its own module where oracle/_ref/refpy is built, else the
+    restatement tests/ref_dpsr.py (pinned to the reference's stored field and gradients by tests/test_dpsr.py)."""
+    ref = load_reference_pymodules()
+    if ref is not None:
+        return ref
+    import types
+    import ref_dpsr
+    return types.SimpleNamespace(dpsr=ref_dpsr)
+
+
+def _load_refpy(refpy):
+    import types
+    from unittest import mock
     for name in ("trimesh", "imageio", "skimage", "skimage.measure", "pytorch3d", "pytorch3d.structures",
                  "pytorch3d.renderer", "igl", "open3d", "plyfile"):
         if name not in sys.modules:

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Deformation-MLP forward+backward: the tcgen05 GEMM chain (utils.time_utils) vs the reference's fp32
+"""Deformation-MLP forward+backward: the wgmma GEMM chain (utils.time_utils) vs the reference's fp32
 PyTorch module (oracle/_ref/refpy/time_utils.py) on the same GPU.  FLOPs per point = 3 124 224
 (SURVEY.md 8(d), blender DeformNetworkNormal, fwd+bwd)."""
 import importlib

@@ -1,16 +1,16 @@
 #!/bin/bash
-# Instruction evidence from the in-tree build (no GPU needed): per kernel, how many tcgen05 / TMA / packed-fp32 /
-# vector-reduction instructions the SASS holds, and the ptxas resource lines.
-#   tools/sass_evidence.sh > profiles/r2_sass_evidence.txt
+# Instruction evidence from the in-tree build (no GPU needed): per kernel, how many wgmma / TMA / vector-reduction
+# instructions the SASS holds, and the ptxas resource lines.
+#   tools/sass_evidence.sh > sass_evidence.txt
 cd "$(dirname "$0")/.."
-echo "# SASS evidence (cuobjdump -sass of the in-tree build, sm_100a): instruction counts per kernel"
+echo "# SASS evidence (cuobjdump -sass of the in-tree build, sm_90a): instruction counts per kernel"
 for o in build/mlp.o build/raster_fwd.o build/raster_bwd.o build/mc.o build/meshrast.o build/densify.o build/loss.o build/dpsr.o build/knn.o; do
   [ -f "$o" ] || continue
   echo "## $o"
   cuobjdump -sass "$o" 2>/dev/null | awk '
     /Function :/ {fn=$3}
-    /UTCHMMA|UTCBAR|UTCATOMSWS|LDTM|UBLKCP|SYNCS|FFMA2|FMUL2|FADD2|REDG|ATOMG|REDUX|MUFU.EX2/ {
-      for (i=1;i<=NF;i++) if ($i ~ /^(UTCHMMA|UTCBAR|UTCATOMSWS|LDTM|UBLKCP|SYNCS|FFMA2|FMUL2|FADD2|REDG|ATOMG|REDUX|MUFU\.EX2)/) {split($i,a,"."); c[fn" "a[1]]++}
+    /HGMMA|WARPGROUP|UBLKCP|SYNCS|REDG|ATOMG|REDUX|MUFU.EX2/ {
+      for (i=1;i<=NF;i++) if ($i ~ /^(HGMMA|WARPGROUP|UBLKCP|SYNCS|REDG|ATOMG|REDUX|MUFU\.EX2)/) {split($i,a,"."); c[fn" "a[1]]++}
     }
     END {for (k in c) printf "  %-90s x%d\n", k, c[k]}' | sort
 done

@@ -128,7 +128,7 @@ def run(a):
         launch.install(REF_TREE)
         resolved = launch.resolved()
     else:
-        # the reference's own stack: its python modules + its stock extensions built for sm_100
+        # the reference's own stack: its python modules + its stock extensions built for sm_90a
         sys.path.insert(0, REF_TREE)
         sys.path.insert(0, os.path.join(ROOT, "oracle", "_ref"))
         resolved = {}
