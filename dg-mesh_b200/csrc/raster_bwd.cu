@@ -6,9 +6,13 @@
 //                          (computeCov2DCUDA + preprocessCUDA, backward.cu:144-396, fused)
 //
 // The reference issues 9 global float atomics per contributing (pixel, Gaussian)
-// pair.  Here each warp (8x4 pixels) reduces its 32 partial gradients with a
-// transposing butterfly (14 shuffles for 9 values), adds the 9 sums into a per-tile
-// shared-memory accumulator, and the tile flushes once per (tile, Gaussian) with
+// pair.  Here the per-Gaussian gradient is written as nine pixel sums over each warp's
+// 8x4 block: six moments of w = G * dL/dG (w, w dx, w dy, w dx^2, w dx dy, w dy^2) and
+// three colour weights.  Each moment is a polynomial in the pixel's offset (u, v) from
+// the block centre, so a lane only stages its two scalars (w, alpha T) per record in
+// shared memory; once per chunk of records the warp contracts them (one record per lane
+// pair, against the fixed u, v and the staged dL/dpixel) and adds the nine sums into a
+// per-tile shared-memory accumulator.  The tile flushes once per (tile, Gaussian) with
 // vector reductions (red.global.add.v4.f32) into a [P,12] accumulator that the fused
 // preprocess-backward consumes and re-zeroes.  The per-pair arithmetic follows the
 // reference's back-to-front recurrence; only the summation order differs (the
@@ -19,62 +23,71 @@
 
 namespace dgm {
 
-#define RB 256
-#define ACC_STRIDE 9
+#define RB 256          // records per TMA batch
+#define ACC_STRIDE 9    // floats per record in the per-tile accumulator
+#define CHUNK 16        // records a warp stages before contracting them
+#define SLOT_F 68       // floats per staged record: w[32], alpha T[32], and 16 B that put the 16 slots in distinct banks
+#define STAGE_BYTES (8 * CHUNK * SLOT_F * 4)  // dynamic shared memory: one staging area per warp
 
-// Reduce the 9 partial gradients of TWO Gaussians (A, B) over the 32 lanes of a warp with a
-// transposing butterfly: at each level a lane keeps half of its values and trades the other
-// half with its partner, so 16 values cost 8+4+2+1+1 = 16 shuffles (+5 for the pair of 9th
-// values) instead of 2 x 9 x 5 = 90 for naive per-value reductions.
-// On return, for lanes with (lane & 1) == 0: r8 = total of value ((lane>>1)&7) of Gaussian
-// (lane>>4); r9 = total of value 8 of Gaussian (lane>>4) on every lane.
-__device__ __forceinline__ void warp_reduce_pair(const float (&vK)[9], const float (&vS)[9], unsigned lane, float& r8,
-                                                 float& r9) {
-  // vK: the 9 values of the Gaussian this lane's half KEEPS (A on lanes 0-15, B on lanes 16-31),
-  // vS: those of the Gaussian it SENDS to the other half -- arranged by the caller, so the first
-  // (widest) butterfly stage needs no selects
-  const unsigned FULL = 0xffffffffu;
-  float a[8];
+// Contract the first n staged records of a warp into s_acc.  Slot k holds w and alpha T of the 32 pixels
+// (pixel = lane of the staging warp: column lane & 7, row lane >> 3) of record `rec` (held by lanes k and
+// k + 16).  Lane l sums slot l & 15 over pixel rows 2h, 2h+1, h = l >> 4, as pixel offsets u, v from the
+// block centre (exact in fp32), then expands the moments about the Gaussian's offset (Gx, Gy) from that
+// centre: sum w dx = Gx S_1 - S_u, sum w dx^2 = Gx^2 S_1 - 2 Gx S_u + S_uu, ...  The two lanes of a slot
+// trade half of their nine partial sums, so each adds 5 or 4 totals (shared-memory float atomics are
+// compare-and-swap loops on sm_90).  Every lane computes; only the lanes of the n filled slots add.
+__device__ __forceinline__ void contract_chunk(const float* stage, const float* dlp, int n, int rec, unsigned lane,
+                                               const float4* geo, float cx, float cy, float* s_acc) {
+  const int k = lane & 15, h = lane >> 4;
+  const float4* w4 = reinterpret_cast<const float4*>(stage + k * SLOT_F + 16 * h);  // w of this half's 16 pixels
+  const float4* a4 = w4 + 8;                                                        // alpha T of the same
+  const float4* d4 = reinterpret_cast<const float4*>(dlp + 16 * h);                 // dlp is [3][32]
+  float c[3];
 #pragma unroll
-  for (int k = 0; k < 8; ++k) a[k] = vK[k] + __shfl_xor_sync(FULL, vS[k], 16);
-  float b[4];
-  {
-    const bool up = lane & 8;
+  for (int i = 0; i < 4; ++i) {
+    const float4 t = a4[i];
+    const float at[4] = {t.x, t.y, t.z, t.w};
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float send = up ? a[k] : a[k + 4];
-      const float keep = up ? a[k + 4] : a[k];
-      b[k] = keep + __shfl_xor_sync(FULL, send, 8);
+    for (int ch = 0; ch < 3; ++ch) {
+      const float4 e = d4[8 * ch + i];
+      const float dl[4] = {e.x, e.y, e.z, e.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) c[ch] = (i == 0 && j == 0) ? at[j] * dl[j] : fmaf(at[j], dl[j], c[ch]);
     }
   }
-  float c[2];
-  {
-    const bool up = lane & 4;
+  // per pixel row r: pixels 8r .. 8r+7 of this half at u = -3.5 .. 3.5, folded about the centre column
+  float sw[2], su[2], suu[2];
 #pragma unroll
-    for (int k = 0; k < 2; ++k) {
-      const float send = up ? b[k] : b[k + 2];
-      const float keep = up ? b[k + 2] : b[k];
-      c[k] = keep + __shfl_xor_sync(FULL, send, 4);
-    }
+  for (int r = 0; r < 2; ++r) {
+    const float4 p = w4[2 * r], q = w4[2 * r + 1];
+    const float w[8] = {p.x, p.y, p.z, p.w, q.x, q.y, q.z, q.w};
+    float a[4], d[4];  // w(u) + w(-u), w(u) - w(-u) for u = m + 0.5
+#pragma unroll
+    for (int m = 0; m < 4; ++m) a[m] = w[4 + m] + w[3 - m], d[m] = w[4 + m] - w[3 - m];
+    sw[r] = (a[0] + a[1]) + (a[2] + a[3]);
+    su[r] = fmaf(3.5f, d[3], fmaf(2.5f, d[2], fmaf(1.5f, d[1], 0.5f * d[0])));
+    suu[r] = fmaf(12.25f, a[3], fmaf(6.25f, a[2], fmaf(2.25f, a[1], 0.25f * a[0])));
   }
-  float d;
-  {
-    const bool up = lane & 2;
-    const float send = up ? c[0] : c[1];
-    const float keep = up ? c[1] : c[0];
-    d = keep + __shfl_xor_sync(FULL, send, 2);
+  const float v0 = 2 * h - 1.5f, v1 = 2 * h - 0.5f;
+  const float S1 = sw[0] + sw[1], Su = su[0] + su[1], Suu = suu[0] + suu[1];
+  const float Sv = fmaf(v1, sw[1], v0 * sw[0]), Suv = fmaf(v1, su[1], v0 * su[0]);
+  const float Svv = fmaf(v1 * v1, sw[1], (v0 * v0) * sw[0]);
+  const float4 g = geo[rec];
+  const float Gx = g.x - cx, Gy = g.y - cy;
+  const float my = fmaf(Gy, S1, -Sv);
+  const float m[10] = {S1, fmaf(Gx, S1, -Su), my, fmaf(Gx, fmaf(Gx, S1, -2.0f * Su), Suu),
+                       fmaf(Gx, my, fmaf(-Gy, Su, Suv)), fmaf(Gy, fmaf(Gy, S1, -2.0f * Sv), Svv),
+                       c[0], c[1], c[2], 0.0f};
+  float* acc = &s_acc[rec * ACC_STRIDE + 5 * h];  // lane h = 0 adds moments 0-4, h = 1 moments 5-8
+#pragma unroll
+  for (int q = 0; q < 5; ++q) {
+    const float keep = h ? m[q + 5] : m[q], send = h ? m[q] : m[q + 5];
+    const float tot = keep + __shfl_xor_sync(0xffffffffu, send, 16);
+    if (k < n && (q < 4 || h == 0)) atomicAdd(&acc[q], tot);
   }
-  d += __shfl_xor_sync(FULL, d, 1);
-  r8 = d;
-  float e = vK[8] + __shfl_xor_sync(FULL, vS[8], 16);
-  e += __shfl_xor_sync(FULL, e, 8);
-  e += __shfl_xor_sync(FULL, e, 4);
-  e += __shfl_xor_sync(FULL, e, 2);
-  e += __shfl_xor_sync(FULL, e, 1);
-  r9 = e;
 }
 
-__global__ void __launch_bounds__(256, 4) render_bwd_kernel(
+__global__ void __launch_bounds__(256, 3) render_bwd_kernel(
     const uint2* __restrict__ ranges, const uint32_t* __restrict__ tile_order, const float4* __restrict__ inst_geo,
     const float4* __restrict__ inst_attr,
     int W, int H, const float* __restrict__ bg_color, const float* __restrict__ final_Ts,
@@ -82,8 +95,10 @@ __global__ void __launch_bounds__(256, 4) render_bwd_kernel(
   __shared__ __align__(128) float4 s_geo[2][RB];
   __shared__ __align__(128) float4 s_attr[2][2 * RB];
   __shared__ float s_acc[RB * ACC_STRIDE];
+  __shared__ __align__(16) float s_dlp[8][3][32];  // dL/dpixel of each warp's 32 pixels, per colour
   __shared__ __align__(8) uint64_t s_bar[2];
   __shared__ int s_maxc;
+  extern __shared__ __align__(16) float s_stage[];  // [8 warps][CHUNK][SLOT_F]
 
   pdl_wait();
   pdl_launch();
@@ -97,6 +112,7 @@ __global__ void __launch_bounds__(256, 4) render_bwd_kernel(
   const uint32_t pix_id = W * py + px;
   const float pixfx = (float)px, pixfy = (float)py;
   const float bx0 = (float)wx0, bx1 = (float)(wx0 + 7), by0 = (float)wy0, by1 = (float)(wy0 + 3);
+  const float cx = wx0 + 3.5f, cy = wy0 + 1.5f;  // centre of the warp's block
   const float2 npx2 = make_float2(-pixfx, -pixfx), npy2 = make_float2(-pixfy, -pixfy);
 
   const uint2 range = ranges[tile];
@@ -141,6 +157,11 @@ __global__ void __launch_bounds__(256, 4) render_bwd_kernel(
     dLp1 = dL_dpixels[1 * HW + pix_id];
     dLp2 = dL_dpixels[2 * HW + pix_id];
   }
+  s_dlp[wid][0][lane] = dLp0;
+  s_dlp[wid][1][lane] = dLp1;
+  s_dlp[wid][2][lane] = dLp2;
+  float* const stage = s_stage + wid * (CHUNK * SLOT_F);
+  int nslot = 0, rec = 0;  // staged records; the record of slot lane & 15
   float bg_dot_dpixel = 0;
   bg_dot_dpixel += bg_color[0] * dLp0;
   bg_dot_dpixel += bg_color[1] * dLp1;
@@ -148,9 +169,6 @@ __global__ void __launch_bounds__(256, 4) render_bwd_kernel(
 
   const float mTb = -T_final * bg_dot_dpixel;  // background term of dL/dalpha, times 1/(1-alpha) per record
   float accum0 = 0.f, accum1 = 0.f, accum2 = 0.f;  // colour composited behind the current record
-  // d(pixel coordinate)/d(NDC), backward.cu:457-458 (double literal 0.5)
-  const float ddelx_dx = 0.5 * W;
-  const float ddely_dy = 0.5 * H;
 
   for (int i = 0; i < rounds; ++i) {
     const int st = i & 1;
@@ -165,8 +183,10 @@ __global__ void __launch_bounds__(256, 4) render_bwd_kernel(
       tma_load_1d(&s_geo[st ^ 1][0], inst_geo + range.x + nlo, ncnt * 16u, &s_bar[st ^ 1]);
       tma_load_1d(&s_attr[st ^ 1][0], inst_attr + 2 * ((size_t)range.x + nlo), ncnt * 32u, &s_bar[st ^ 1]);
     }
-    // ---- cull (same conservative extent test as the forward pass)
-    unsigned keep[RB / 32];
+    // ---- cull (same conservative extent test as the forward pass); lane k keeps the ballot of
+    // records [32k, 32k + 32), so that the k loop below stays rolled and its body (with the
+    // contraction) is emitted once
+    unsigned keep_k = 0;
 #pragma unroll
     for (int k = 0; k < RB / 32; ++k) {
       const int r = k * 32 + lane;
@@ -174,17 +194,17 @@ __global__ void __launch_bounds__(256, 4) render_bwd_kernel(
       if (r < cnt && (lo + r) < wmax) {
         kp = cull_keep(s_geo[st][r], s_attr[st][2 * r], bx0, bx1, by0, by1);
       }
-      keep[k] = __ballot_sync(0xffffffffu, kp);
+      const unsigned b = __ballot_sync(0xffffffffu, kp);
+      if (lane == k) keep_k = b;
     }
-    // ---- back to front, two records per iteration (two-lane quadratic form, one
-    // butterfly reduction for both).  A is the record nearer the back (processed first).
-    // Per lane only MOMENTS of w = G * dL/dG are accumulated (w, w dx, w dy, w dx^2, w dx dy,
-    // w dy^2) plus the colour weights; the per-Gaussian factors (conic, opacity, viewport
-    // scale) are applied once per (tile, Gaussian) at flush time.  Branch-free: inactive
-    // lanes are masked with selects.
-#pragma unroll
+    // ---- back to front, two records per iteration (two-lane quadratic form).  A is the record
+    // nearer the back (processed first).  Per lane only w = G * dL/dG and alpha T are formed and
+    // staged; the moments are formed by contract_chunk, the per-Gaussian factors (conic, opacity,
+    // viewport scale) once per (tile, Gaussian) at flush time.  Branch-free: inactive lanes are
+    // masked with selects.
+#pragma unroll 1
     for (int k = RB / 32 - 1; k >= 0; --k) {
-      unsigned mask = keep[k];
+      unsigned mask = __shfl_sync(0xffffffffu, keep_k, k);
       while (mask) {
         const int bA = 31 - __clz(mask);
         mask &= ~(1u << bA);
@@ -204,8 +224,6 @@ __global__ void __launch_bounds__(256, 4) render_bwd_kernel(
         m3 = mul2_rn(dy2, m3);
         const float2 npow = fma2_rn(sq, make_float2(0.5f, 0.5f), m3);  // = -power
         // order-dependent part (scalar): transmittance and the colour behind each record
-        float wq[2], atq[2];
-        bool contrib = false;
 #pragma unroll
         for (int q = 0; q < 2; ++q) {
           const float np = q ? npow.y : npow.x;
@@ -217,7 +235,6 @@ __global__ void __launch_bounds__(256, 4) render_bwd_kernel(
           const float G = expf(-np);
           const float alpha = fminf(0.99f, opac * G);
           const bool act = pre && !(alpha < 1.0f / 255.0f);
-          contrib |= act;
           const float r = __fdividef(1.0f, 1.0f - alpha);
           const float a_eff = act ? alpha : 0.0f;  // inactive lanes leave every state variable unchanged
           T *= act ? r : 1.0f;
@@ -226,46 +243,31 @@ __global__ void __launch_bounds__(256, 4) render_bwd_kernel(
           dLa = fmaf(d1, dLp1, dLa);
           dLa = fmaf(d2, dLp2, dLa);
           dLa = fmaf(dLa, T, mTb * r);
-          wq[q] = act ? (G * opac) * dLa : 0.0f;
-          atq[q] = a_eff * T;
+          const float w = act ? (G * opac) * dLa : 0.0f;
           // colour behind the NEXT record: alpha c + (1 - alpha) accum  (backward.cu:507, evaluated eagerly)
           accum0 = fmaf(a_eff, d0, accum0);
           accum1 = fmaf(a_eff, d1, accum1);
           accum2 = fmaf(a_eff, d2, accum2);
+          // only records with a contributing lane take a slot (the others add exact zeros)
+          if (__any_sync(0xffffffffu, act)) {
+            stage[nslot * SLOT_F + lane] = w;
+            stage[nslot * SLOT_F + 32 + lane] = a_eff * T;
+            if ((int)(lane & 15) == nslot) rec = j;
+            ++nslot;
+          }
         }
-        // moments of w for both records at once (packed).  Component .x is the record this lane's half
-        // keeps in the reduction (A on lanes 0-15, B on lanes 16-31), .y the one it hands over.
-        float v[2][9];
-        {
-          const bool up = lane & 16;
-          const float2 w2 = up ? make_float2(wq[1], wq[0]) : make_float2(wq[0], wq[1]);
-          const float2 at2 = up ? make_float2(atq[1], atq[0]) : make_float2(atq[0], atq[1]);
-          const float2 ex2 = up ? make_float2(dx2.y, dx2.x) : dx2;
-          const float2 ey2 = up ? make_float2(dy2.y, dy2.x) : dy2;
-          const float2 wx = mul2_rn(w2, ex2), wy = mul2_rn(w2, ey2);
-          const float2 wxx = mul2_rn(wx, ex2), wxy = mul2_rn(wx, ey2), wyy = mul2_rn(wy, ey2);
-          const float2 c0 = mul2_rn(at2, make_float2(dLp0, dLp0)), c1 = mul2_rn(at2, make_float2(dLp1, dLp1)),
-                       c2 = mul2_rn(at2, make_float2(dLp2, dLp2));
-          v[0][0] = w2.x, v[1][0] = w2.y;
-          v[0][1] = wx.x, v[1][1] = wx.y;
-          v[0][2] = wy.x, v[1][2] = wy.y;
-          v[0][3] = wxx.x, v[1][3] = wxx.y;
-          v[0][4] = wxy.x, v[1][4] = wxy.y;
-          v[0][5] = wyy.x, v[1][5] = wyy.y;
-          v[0][6] = c0.x, v[1][6] = c0.y;
-          v[0][7] = c1.x, v[1][7] = c1.y;
-          v[0][8] = c2.x, v[1][8] = c2.y;
-        }
-        if (__any_sync(0xffffffffu, contrib)) {
-          float r8, r9;
-          warp_reduce_pair(v[0], v[1], lane, r8, r9);
-          const int jj = (lane & 16) ? jB : jA;
-          float* acc = &s_acc[jj * ACC_STRIDE];
-          // a lone record (two == false) reduces against zeros: only its own half is added
-          if ((lane & 1) == 0 && (two || !(lane & 16))) atomicAdd(&acc[(lane >> 1) & 7], r8);
-          if ((lane & 15) == 1 && (two || !(lane & 16))) atomicAdd(&acc[8], r9);
+        if (nslot > CHUNK - 2) {  // no room for another pair
+          __syncwarp();
+          contract_chunk(stage, &s_dlp[wid][0][0], nslot, rec, lane, s_geo[st], cx, cy, s_acc);
+          __syncwarp();
+          nslot = 0;
         }
       }
+    }
+    if (nslot > 0) {  // the batch's records must be in s_acc before the flush
+      __syncwarp();
+      contract_chunk(stage, &s_dlp[wid][0][0], nslot, rec, lane, s_geo[st], cx, cy, s_acc);
+      nslot = 0;
     }
     __syncthreads();
     // ---- flush this batch: one vector reduction triple per (tile, Gaussian)
@@ -281,6 +283,9 @@ __global__ void __launch_bounds__(256, 4) render_bwd_kernel(
       }
       if (nz) {
         // moments -> gradients (backward.cu:531-554): a[0..5] = sums of w, w dx, w dy, w dx^2, w dx dy, w dy^2
+        // d(pixel coordinate)/d(NDC), backward.cu:457-458 (double literal 0.5)
+        const float ddelx_dx = 0.5 * W;
+        const float ddely_dy = 0.5 * H;
         const float4 con_o = s_attr[st][2 * tid];
         const uint32_t id = __float_as_uint(s_attr[st][2 * tid + 1].w);
         const float g_mx = -ddelx_dx * (con_o.x * a[1] + con_o.y * a[2]);
@@ -621,6 +626,13 @@ cudaError_t launch_backward(const BwdArgs& a, cudaStream_t s) {
 
 // gradient of the alpha-compositing (fills the GPU); leaves the per-Gaussian moments in grad_acc
 cudaError_t launch_render_bwd(const BwdArgs& a, cudaStream_t s) {
+  static unsigned long long attr = 0;  // per device
+  if (once_per_device(attr)) {
+    // the staging area takes the kernel past 48 KB of shared memory; 3 CTAs per SM need the largest carveout
+    cudaFuncSetAttribute(render_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, STAGE_BYTES);
+    cudaFuncSetAttribute(render_bwd_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+                         cudaSharedmemCarveoutMaxShared);
+  }
   if (a.P == 0) return cudaSuccess;
   const unsigned gx = (a.W + TILE_X - 1) / TILE_X, gy = (a.H + TILE_Y - 1) / TILE_Y;
   const int T = gx * gy;
@@ -628,7 +640,7 @@ cudaError_t launch_render_bwd(const BwdArgs& a, cudaStream_t s) {
   ImgWS im = ImgWS::from((char*)a.img_ws, (size_t)a.W * a.H, T);
   BinWS b = BinWS::from((char*)a.binning_ws, (size_t)a.R_cap);
   g_prof.begin(5, s);
-  launch_pdl(render_bwd_kernel, dim3(T), dim3(256), 0, s, (const uint2*)im.ranges, (const uint32_t*)im.tile_order,
+  launch_pdl(render_bwd_kernel, dim3(T), dim3(256), STAGE_BYTES, s, (const uint2*)im.ranges, (const uint32_t*)im.tile_order,
              (const float4*)b.inst_geo, (const float4*)b.inst_attr, a.W, a.H, a.background, (const float*)im.final_T,
              (const uint32_t*)im.n_contrib, a.dL_dpix, g.grad_acc);
   g_prof.end(5, s);
