@@ -166,17 +166,18 @@ int dgr_backward(int P, int D, int M, const float* background, int W, int H, con
   a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.scales = scales;
   a.scale_modifier = scale_modifier; a.rotations = rotations; a.cov3D_precomp = cov3D_precomp;
   a.viewmatrix = viewmatrix; a.projmatrix = projmatrix; a.cam_pos = cam_pos;
-  a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy; a.radii = radii;
+  a.tan_fovx = &tan_fovx; a.tan_fovy = &tan_fovy; a.radii = radii;
   a.geom_ws = geom_ws; a.binning_ws = binning_ws; a.img_ws = img_ws; a.R_cap = R_cap;
   a.dL_dpix = dL_dpix; a.dL_dmean2D = dL_dmean2D; a.dL_dconic = dL_dconic; a.dL_dopacity = dL_dopacity;
   a.dL_dcolor = dL_dcolor; a.dL_dmean3D = dL_dmean3D; a.dL_dcov3D = dL_dcov3D; a.dL_dsh = dL_dsh;
-  a.dL_dscale = dL_dscale; a.dL_drot = dL_drot; a.accumulate = 0;
+  a.dL_dscale = dL_dscale; a.dL_drot = dL_drot;
+  a.F = 1; a.per_frame = 0; a.geom_stride = 0;
   return check(dgm::launch_backward(a, (cudaStream_t)stream));
 }
 
 namespace {
 // Internal streams for the frame batches (created once per process).
-//   hi[]  high priority: the short, latency-bound kernels (preprocess / binning / sort, preprocess_bwd)
+//   hi[]  high priority: the short, latency-bound kernels (preprocess / binning / sort)
 //   lo[]  low priority : the blend kernels, each of which fills the GPU on its own; two streams,
 //         alternating frames, so the next kernel's CTAs fill the SMs while the previous one's tail drains
 // A frame's binning chain runs on hi[f % NH] and its blend kernel on lo behind an event.  The block
@@ -186,7 +187,7 @@ namespace {
 struct BatchStreams {
   static const int NH = 4;
   cudaStream_t hi[NH] = {}, lo[2] = {};
-  cudaEvent_t fork = nullptr, done_hi[NH] = {}, done_lo[2] = {}, ready[NH] = {}, blended[2] = {};
+  cudaEvent_t fork = nullptr, done_hi[NH] = {}, done_lo[2] = {}, ready[NH] = {};
   bool ok = false;
   std::mutex mu;  // one batch call at a time per device (the events above are shared)
   bool init() {
@@ -202,7 +203,6 @@ struct BatchStreams {
     for (int i = 0; i < 2; ++i) {
       if (cudaStreamCreateWithPriority(&lo[i], cudaStreamNonBlocking, least) != cudaSuccess) return false;
       if (cudaEventCreateWithFlags(&done_lo[i], cudaEventDisableTiming) != cudaSuccess) return false;
-      if (cudaEventCreateWithFlags(&blended[i], cudaEventDisableTiming) != cudaSuccess) return false;
     }
     ok = true;
     return true;
@@ -333,73 +333,50 @@ int dgr_backward_batch(int F, int P, int D, int M, const float* background, int 
                        float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
                        int n_streams, void* stream) {
   if (F <= 0 || P < 0 || W <= 0 || H <= 0 || R_cap < 0) return bad("dgr_backward_batch: bad size");
+  if (F > PB_MAX_FRAMES) return bad("dgr_backward_batch: more than 64 frames");
   if (P == 0) return DGM_OK;
   if (!background || !means3D || !viewmatrices || !projmatrices || !cam_poses || !tan_fovx_host || !tan_fovy_host ||
-      !geom_ws || !binning_ws || !img_ws || !dL_dpix || !dL_dmean2D || !dL_dopacity || !dL_dcolor || !dL_dmean3D ||
-      !dL_dcov3D || !dL_dscale || !dL_drot || (shs && !dL_dsh))
+      !geom_ws || !binning_ws || !img_ws || !dL_dpix || !dL_dmean2D || !dL_dopacity || (!shs && !dL_dcolor) ||
+      !dL_dmean3D || (cov3D_precomp && !dL_dcov3D) || !dL_dscale || !dL_drot || (shs && !dL_dsh))
     return bad("dgr_backward_batch: null required pointer");
-  // render_bwd kernels serialise on the low-priority stream; every preprocess_bwd goes to ONE
-  // high-priority stream (they accumulate into the same buffers, so they must stay ordered) and
-  // overlaps the render_bwd of the next frame
+  // the render_bwd kernels alternate two low-priority streams (the next one's CTAs fill the SMs while the
+  // previous one's tail drains); one per-Gaussian kernel for all frames follows once both have finished
   const bool multi = n_streams > 1 && F > 1;
   cudaStream_t main_s = (cudaStream_t)stream;
-  cudaStream_t s_pp = main_s;
   BatchStreams* bs = nullptr;
   std::unique_lock<std::mutex> lk;
   if (multi) {
     bs = batch_streams();
     if (!bs) return check(cudaGetLastError());
     lk = std::unique_lock<std::mutex>(bs->mu);
-    s_pp = bs->hi[0];
     cudaEventRecord(bs->fork, main_s);
     for (int i = 0; i < 2; ++i) cudaStreamWaitEvent(bs->lo[i], bs->fork, 0);
-    cudaStreamWaitEvent(s_pp, bs->fork, 0);
   }
-  auto pf = [&](const float* p, int bit, size_t width, int f) {
-    return (p && (per_frame & bit)) ? p + (size_t)f * P * width : p;
-  };
-  auto pfo = [&](float* p, int bit, size_t width, int f) {
-    return (p && (per_frame & bit)) ? p + (size_t)f * P * width : p;
-  };
-  const size_t cw = shs ? (size_t)M * 3 : 3;
+  dgm::BwdArgs a;
+  a.P = P; a.D = D; a.M = M; a.background = background; a.W = W; a.H = H;
+  a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.scales = scales;
+  a.scale_modifier = scale_modifier; a.rotations = rotations; a.cov3D_precomp = cov3D_precomp;
+  a.viewmatrix = viewmatrices; a.projmatrix = projmatrices; a.cam_pos = cam_poses;
+  a.tan_fovx = tan_fovx_host; a.tan_fovy = tan_fovy_host; a.radii = radii;
+  a.geom_ws = geom_ws; a.binning_ws = binning_ws; a.img_ws = img_ws; a.R_cap = R_cap; a.dL_dpix = dL_dpix;
+  a.dL_dmean2D = dL_dmean2D; a.dL_dconic = nullptr; a.dL_dopacity = dL_dopacity; a.dL_dcolor = dL_dcolor;
+  a.dL_dmean3D = dL_dmean3D; a.dL_dcov3D = dL_dcov3D; a.dL_dsh = dL_dsh;
+  a.dL_dscale = dL_dscale; a.dL_drot = dL_drot;
+  a.F = F; a.per_frame = per_frame; a.geom_stride = geom_stride;
   cudaError_t e = cudaSuccess;
   for (int f = 0; f < F && e == cudaSuccess; ++f) {
-    dgm::BwdArgs a;
-    a.P = P; a.D = D; a.M = M; a.background = background; a.W = W; a.H = H;
-    a.means3D = pf(means3D, DGR_PF_MEANS, 3, f); a.shs = pf(shs, DGR_PF_COLOR, cw, f);
-    a.colors_precomp = pf(colors_precomp, DGR_PF_COLOR, 3, f); a.scales = pf(scales, DGR_PF_SCALES, 3, f);
-    a.scale_modifier = scale_modifier; a.rotations = pf(rotations, DGR_PF_ROTS, 4, f);
-    a.cov3D_precomp = pf(cov3D_precomp, DGR_PF_COV, 6, f);
-    a.viewmatrix = viewmatrices + 16 * f; a.projmatrix = projmatrices + 16 * f; a.cam_pos = cam_poses + 3 * f;
-    a.tan_fovx = tan_fovx_host[f]; a.tan_fovy = tan_fovy_host[f];
-    a.radii = radii ? radii + (size_t)f * P : nullptr;
-    a.geom_ws = (char*)geom_ws + f * geom_stride; a.binning_ws = (char*)binning_ws + f * binning_stride;
-    a.img_ws = (char*)img_ws + f * img_stride; a.R_cap = R_cap;
-    a.dL_dpix = dL_dpix + (size_t)f * 3 * W * H;
-    a.dL_dmean2D = dL_dmean2D + (size_t)f * P * 3; a.dL_dconic = nullptr;
-    a.dL_dopacity = pfo(dL_dopacity, DGR_PF_OPAC, 1, f);
-    a.dL_dcolor = pfo(dL_dcolor, shs ? 0 : DGR_PF_COLOR, 3, f);  // with SH colours dL_dcolor is scratch
-    a.dL_dmean3D = pfo(dL_dmean3D, DGR_PF_MEANS, 3, f); a.dL_dcov3D = pfo(dL_dcov3D, DGR_PF_COV, 6, f);
-    a.dL_dsh = pfo(dL_dsh, DGR_PF_COLOR, cw, f); a.dL_dscale = pfo(dL_dscale, DGR_PF_SCALES, 3, f);
-    a.dL_drot = pfo(dL_drot, DGR_PF_ROTS, 4, f);
-    // shared inputs: the first frame writes, later frames add; per-frame inputs: always written
-    a.accumulate = (f > 0) ? (DGR_PF_ALL & ~per_frame) : 0;
-    cudaStream_t s_blend = multi ? bs->lo[f & 1] : main_s;
-    e = dgm::launch_render_bwd(a, s_blend);
-    if (multi) {
-      cudaEventRecord(bs->blended[f & 1], s_blend);
-      cudaStreamWaitEvent(s_pp, bs->blended[f & 1], 0);
-    }
-    if (e == cudaSuccess) e = dgm::launch_preprocess_bwd(a, s_pp);
+    dgm::BwdArgs af = a;  // launch_render_bwd reads frame 0 of its arguments
+    af.geom_ws = (char*)geom_ws + f * geom_stride; af.binning_ws = (char*)binning_ws + f * binning_stride;
+    af.img_ws = (char*)img_ws + f * img_stride; af.dL_dpix = dL_dpix + (size_t)f * 3 * W * H;
+    e = dgm::launch_render_bwd(af, multi ? bs->lo[f & 1] : main_s);
   }
   if (multi) {
     for (int i = 0; i < 2; ++i) {
       cudaEventRecord(bs->done_lo[i], bs->lo[i]);
       cudaStreamWaitEvent(main_s, bs->done_lo[i], 0);
     }
-    cudaEventRecord(bs->done_hi[0], s_pp);
-    cudaStreamWaitEvent(main_s, bs->done_hi[0], 0);
   }
+  if (e == cudaSuccess) e = dgm::launch_preprocess_bwd(a, main_s);
   return check(e != cudaSuccess ? e : cudaGetLastError());
 }
 

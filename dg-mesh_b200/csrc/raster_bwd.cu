@@ -3,7 +3,8 @@
 //   render_bwd_kernel      gradient of the alpha-composite (role of renderCUDA,
 //                          dgr/cuda_rasterizer/backward.cu:399-557)
 //   preprocess_bwd_kernel  chain rule to means3D / scales / rotations / SH / opacity
-//                          (computeCov2DCUDA + preprocessCUDA, backward.cu:144-396, fused)
+//                          (computeCov2DCUDA + preprocessCUDA, backward.cu:144-396, fused), one
+//                          launch for all frames of a batch
 //
 // The reference issues 9 global float atomics per contributing (pixel, Gaussian)
 // pair.  Here the per-Gaussian gradient is written as nine pixel sums over each warp's
@@ -17,6 +18,7 @@
 // preprocess-backward consumes and re-zeroes.  The per-pair arithmetic follows the
 // reference's back-to-front recurrence; only the summation order differs (the
 // reference's own order is non-deterministic).
+#include "../../include/dgmesh_b200.h"
 #include "common.cuh"
 #include "raster_math.cuh"
 #include "raster_kernels.h"
@@ -301,18 +303,18 @@ __global__ void __launch_bounds__(256, 3) render_bwd_kernel(
 }
 
 // ===================================================== preprocess (bwd) ====
-// SH colour gradient (backward.cu:20-139): returns dL/d(mean) contribution, writes dL_dsh.
+// SH colour gradient (backward.cu:20-139): returns dL/d(mean) contribution.  dL/dsh is the outer product
+// dL_dsh[k][ch] = w[k] * dRGB[ch] (w[k] = 0 for k >= (deg + 1)^2); the caller forms it from the two factors.
 __device__ __forceinline__ float3 sh_backward(int deg, const float3 pos, const float3 campos, const float* sh,
-                                              const uint8_t* clamped, const float3 dL_dcolor, float* dL_dsh) {
+                                              const uint8_t* clamped, const float3 dL_dcolor, float* w /*[16]*/,
+                                              float* dRGB /*[3]*/) {
   const float3 dir_orig = make_float3(pos.x - campos.x, pos.y - campos.y, pos.z - campos.z);
   const float len = sqrtf(dir_orig.x * dir_orig.x + dir_orig.y * dir_orig.y + dir_orig.z * dir_orig.z);
   const float x = dir_orig.x / len, y = dir_orig.y / len, z = dir_orig.z / len;
-  float dRGB[3] = {dL_dcolor.x, dL_dcolor.y, dL_dcolor.z};
-  dRGB[0] *= clamped[0] ? 0 : 1;
-  dRGB[1] *= clamped[1] ? 0 : 1;
-  dRGB[2] *= clamped[2] ? 0 : 1;
+  dRGB[0] = dL_dcolor.x * (clamped[0] ? 0 : 1);
+  dRGB[1] = dL_dcolor.y * (clamped[1] ? 0 : 1);
+  dRGB[2] = dL_dcolor.z * (clamped[2] ? 0 : 1);
   float ddir[3] = {0.f, 0.f, 0.f};  // dL/d(dir) accumulated over channels
-  float w[16];
 #pragma unroll
   for (int k = 0; k < 16; ++k) w[k] = 0.f;
   w[0] = kSH0;
@@ -340,13 +342,6 @@ __device__ __forceinline__ float3 sh_backward(int deg, const float3 pos, const f
       }
     }
   }
-  const int ncoef = (deg + 1) * (deg + 1);
-#pragma unroll
-  for (int k = 0; k < 16; ++k) {
-#pragma unroll
-    for (int ch = 0; ch < 3; ++ch) dL_dsh[k * 3 + ch] = (k < ncoef) ? w[k] * dRGB[ch] : 0.f;
-  }
-
 #pragma unroll
   for (int ch = 0; ch < 3; ++ch) {
     float dx = 0.f, dy = 0.f, dz = 0.f;
@@ -390,232 +385,315 @@ __device__ __forceinline__ float3 sh_backward(int deg, const float3 pos, const f
   return r;
 }
 
-// write v, or add it to what the buffer holds (never reads the buffer unless accumulating)
-__device__ __forceinline__ void acc_store(float* p, float v, int accumulate) { *p = accumulate ? *p + v : v; }
+// ---- per-Gaussian backward of a frame batch (F = 1: one frame).  A block covers NG Gaussians x FB frames per
+// pass (FB * NG = 256): warp w takes 32 consecutive Gaussians of frame f0 + w % FB, so per-frame slabs load
+// and store coalesced.  Gradients of per-frame inputs are written by the frame's thread.  Gradients of inputs
+// shared by the frames are staged per (frame, Gaussian) in shared memory and summed over the frames in frame
+// order f = 0, 1, ..., F - 1 (the rounding of F - 1 sequential fp32 additions), then written once per pass.
+// The SH gradient is staged as its two factors w[16], dRGB[3] and the products are formed by the summing
+// thread; for shared SH the coefficients of a Gaussian come from HBM once and from L1/L2 for the other frames.
+// staging slots: the SH factors w[16] and dRGB[3], opacity, colour, mean, scale, rotation, cov3D
+#define SL_W 0
+#define SL_RGB 16
+#define SL_OPAC 19
+#define SL_COL 20
+#define SL_MEAN 23
+#define SL_SCALE 26
+#define SL_ROT 29
+#define SL_COV 33
+#define SL_COUNT 39
 
-// `accumulate` bits (DGR_PF_* of include/dgmesh_b200.h): which parameter-gradient outputs are summed
-#define ACC_MEANS 1
-#define ACC_SCALES 2
-#define ACC_ROTS 4
-#define ACC_OPAC 8
-#define ACC_COLOR 16  // dL_dsh / dL_dcolor
-#define ACC_COV 32
-#define ACC_ALL 63
+// frames per pass of a 256-thread block (one frame: any block size)
+static __host__ __device__ inline int pb_frames_per_pass(int F) { return F >= 8 ? 8 : F >= 4 ? 4 : F >= 2 ? 2 : 1; }
 
-__global__ void __launch_bounds__(128) preprocess_bwd_kernel(
-    int P, int D, int M, const float* __restrict__ means3D, const int* __restrict__ radii,
+struct PbCams {  // per frame: tan(fov / 2) and focal lengths in pixels
+  float tanx[PB_MAX_FRAMES], tany[PB_MAX_FRAMES], fx[PB_MAX_FRAMES], fy[PB_MAX_FRAMES];
+};
+
+// NT threads per block.  One frame (no staging) runs as 128-thread blocks, 3 per SM (the register budget of the
+// one-frame math without a cap); a batch as 256-thread blocks, 2 per SM, 128 registers, 8 frames per pass.
+template <int NT, int MIN_BLOCKS>
+__global__ void __launch_bounds__(NT, MIN_BLOCKS) preprocess_bwd_kernel(
+    int F, int P, int D, int M, int per_frame, const float* __restrict__ means3D, const int* __restrict__ radii,
     const float* __restrict__ shs, const float* __restrict__ scales, const float* __restrict__ rotations,
-    float scale_modifier, const float* __restrict__ cov3D_precomp, const float* __restrict__ view,
-    const float* __restrict__ proj, float focal_x, float focal_y, float tan_fovx, float tan_fovy,
-    const float* __restrict__ cam_pos, GeomWS g, float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic,
+    float scale_modifier, const float* __restrict__ cov3D_precomp, const float* __restrict__ views,
+    const float* __restrict__ projs, const float* __restrict__ cam_poses, const PbCams cams, char* geom_ws,
+    size_t geom_stride, float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic,
     float* __restrict__ dL_dopacity, float* __restrict__ dL_dcolor, float* __restrict__ dL_dmean3D,
     float* __restrict__ dL_dcov3D, float* __restrict__ dL_dsh, float* __restrict__ dL_dscale,
-    float* __restrict__ dL_drot, int accumulate) {
+    float* __restrict__ dL_drot) {
+  constexpr int PB_STRIDE = NT + 1;  // floats per staging slot: NT (frame, Gaussian) values, + 1 so that slot k starts in bank k
+  __shared__ float s_stage[SL_COUNT * PB_STRIDE];
   pdl_wait();
   pdl_launch();
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= P) return;
-  const bool visible = radii[idx] > 0;
-  // fetch + clear the accumulators written by render_bwd_kernel
-  const float4 a0 = g.grad_acc[3 * idx + 0], a1 = g.grad_acc[3 * idx + 1], a2 = g.grad_acc[3 * idx + 2];
-  g.grad_acc[3 * idx + 0] = make_float4(0, 0, 0, 0);
-  g.grad_acc[3 * idx + 1] = make_float4(0, 0, 0, 0);
-  g.grad_acc[3 * idx + 2] = make_float4(0, 0, 0, 0);
-  const float2 dm2 = make_float2(a0.x, a0.y);
-  const float3 dcon = make_float3(a0.z, a0.w, a1.x);  // (xx, xy, yy) slots .x .y .w of the reference float4
-  const float dop = a1.y;
-  const float3 dcol = make_float3(a1.z, a1.w, a2.x);
+  const int FB = pb_frames_per_pass(F), NG = NT / FB;
+  const int tid = threadIdx.x, wid = tid >> 5;
+  const int fi = wid % FB, gl = (wid / FB) * 32 + (tid & 31);
+  const int g0 = blockIdx.x * NG, g = g0 + gl;
+  // outputs summed over the frames (DGR_PF_* bits; with one frame every output is that frame's).  dL_dcolor
+  // follows the colour input's bit, except with SH colours, where it is [P,3] scratch
+  const int sum = F > 1 ? (DGR_PF_ALL & ~per_frame) : 0;
+  const bool sum_col = dL_dcolor && F > 1 && (shs || (sum & DGR_PF_COLOR));
+  const bool sum_sh = shs && (sum & DGR_PF_COLOR);
+  const int ncoef = (D + 1) * (D + 1);
+  float* const stage = s_stage + fi * NG + gl;
 
-  dL_dmean2D[3 * idx + 0] = dm2.x;
-  dL_dmean2D[3 * idx + 1] = dm2.y;
-  dL_dmean2D[3 * idx + 2] = 0.f;
-  if (dL_dconic) reinterpret_cast<float4*>(dL_dconic)[idx] = make_float4(dcon.x, dcon.y, 0.f, dcon.z);
-  // parameter gradients: written, or (frame batches) added to the running sum over frames
-  if (accumulate == ACC_ALL && !visible) return;  // a culled Gaussian adds nothing
-  acc_store(&dL_dopacity[idx], dop, accumulate & ACC_OPAC);
-  acc_store(&dL_dcolor[3 * idx + 0], dcol.x, accumulate & ACC_COLOR);
-  acc_store(&dL_dcolor[3 * idx + 1], dcol.y, accumulate & ACC_COLOR);
-  acc_store(&dL_dcolor[3 * idx + 2], dcol.z, accumulate & ACC_COLOR);
+  for (int f0 = 0; f0 < F; f0 += FB) {
+    const int f = f0 + fi;
+    if (f < F && g < P) {
+      const size_t fg = (size_t)f * P + g;
+      auto slab = [&](const float* p, int bit, int width) {
+        return (per_frame & bit) ? p + (size_t)f * P * width : p;
+      };
+      // staged when summed over the frames, else written to frame f's slab
+      auto put = [&](bool summed, float* out, int width, int slot, int c, float v) {
+        if (summed) stage[(slot + c) * PB_STRIDE] = v;
+        else out[fg * width + c] = v;
+      };
+      const GeomWS gw = GeomWS::from(geom_ws + f * geom_stride, P);
+      const bool visible = (radii ? radii[fg] : gw.radii[g]) > 0;
+      // fetch + clear the accumulators written by render_bwd_kernel
+      const float4 a0 = gw.grad_acc[3 * g + 0], a1 = gw.grad_acc[3 * g + 1], a2 = gw.grad_acc[3 * g + 2];
+      gw.grad_acc[3 * g + 0] = make_float4(0, 0, 0, 0);
+      gw.grad_acc[3 * g + 1] = make_float4(0, 0, 0, 0);
+      gw.grad_acc[3 * g + 2] = make_float4(0, 0, 0, 0);
+      const float2 dm2 = make_float2(a0.x, a0.y);
+      const float3 dcon = make_float3(a0.z, a0.w, a1.x);  // (xx, xy, yy) slots .x .y .w of the reference float4
+      const float dop = a1.y;
+      const float3 dcol = make_float3(a1.z, a1.w, a2.x);
 
-  float dcov[6] = {0, 0, 0, 0, 0, 0};
-  float3 dmean = make_float3(0, 0, 0);
-  float3 dscale = make_float3(0, 0, 0);
-  float4 drot = make_float4(0, 0, 0, 0);
-
-  if (!visible) {
-    if (dL_dsh && !(accumulate & ACC_COLOR)) {
-      float* dst = dL_dsh + (size_t)idx * M * 3;
-      if (M == 16) {
-#pragma unroll
-        for (int i = 0; i < 12; ++i) reinterpret_cast<float4*>(dst)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      } else {
-        for (int k = 0; k < M * 3; ++k) dst[k] = 0.f;
+      dL_dmean2D[3 * fg + 0] = dm2.x;
+      dL_dmean2D[3 * fg + 1] = dm2.y;
+      dL_dmean2D[3 * fg + 2] = 0.f;
+      if (dL_dconic) reinterpret_cast<float4*>(dL_dconic)[fg] = make_float4(dcon.x, dcon.y, 0.f, dcon.z);
+      put(sum & DGR_PF_OPAC, dL_dopacity, 1, SL_OPAC, 0, dop);
+      if (dL_dcolor) {
+        put(sum_col, dL_dcolor, 3, SL_COL, 0, dcol.x);
+        put(sum_col, dL_dcolor, 3, SL_COL, 1, dcol.y);
+        put(sum_col, dL_dcolor, 3, SL_COL, 2, dcol.z);
       }
-    }
-  } else {
-    const float3 mean = make_float3(means3D[3 * idx], means3D[3 * idx + 1], means3D[3 * idx + 2]);
-    const float* cov3D = cov3D_precomp ? cov3D_precomp + 6 * idx : g.cov3D + 6 * idx;
-    // ---------------- gradient through the 2D covariance / conic (backward.cu:144-274)
-    EwaFrame fr;
-    ewa_frame(mean, focal_x, focal_y, tan_fovx, tan_fovy, cov3D, view, fr);
-    const float limx = 1.3f * tan_fovx, limy = 1.3f * tan_fovy;
-    const float x_grad_mul = fr.txtz < -limx || fr.txtz > limx ? 0 : 1;
-    const float y_grad_mul = fr.tytz < -limy || fr.tytz > limy ? 0 : 1;
-    const float3 c2 = ewa_cov2d(fr);
-    const float a = c2.x, b = c2.y, c = c2.z;
-    const float denom = a * c - b * b;
-    float dL_da = 0, dL_db = 0, dL_dc = 0;
-    const float denom2inv = 1.0f / ((denom * denom) + 0.0000001f);
-    const Mat3& T = fr.T;
-    const Mat3& Vrk = fr.Vrk;
-    if (denom2inv != 0) {
-      dL_da = denom2inv * (-c * c * dcon.x + 2 * b * c * dcon.y + (denom - a * c) * dcon.z);
-      dL_dc = denom2inv * (-a * a * dcon.z + 2 * a * b * dcon.y + (denom - a * c) * dcon.x);
-      dL_db = denom2inv * 2 * (b * c * dcon.x - (denom + 2 * b * b) * dcon.y + a * b * dcon.z);
-      dcov[0] = (T.c[0][0] * T.c[0][0] * dL_da + T.c[0][0] * T.c[1][0] * dL_db + T.c[1][0] * T.c[1][0] * dL_dc);
-      dcov[3] = (T.c[0][1] * T.c[0][1] * dL_da + T.c[0][1] * T.c[1][1] * dL_db + T.c[1][1] * T.c[1][1] * dL_dc);
-      dcov[5] = (T.c[0][2] * T.c[0][2] * dL_da + T.c[0][2] * T.c[1][2] * dL_db + T.c[1][2] * T.c[1][2] * dL_dc);
-      dcov[1] = 2 * T.c[0][0] * T.c[0][1] * dL_da + (T.c[0][0] * T.c[1][1] + T.c[0][1] * T.c[1][0]) * dL_db +
-                2 * T.c[1][0] * T.c[1][1] * dL_dc;
-      dcov[2] = 2 * T.c[0][0] * T.c[0][2] * dL_da + (T.c[0][0] * T.c[1][2] + T.c[0][2] * T.c[1][0]) * dL_db +
-                2 * T.c[1][0] * T.c[1][2] * dL_dc;
-      dcov[4] = 2 * T.c[0][2] * T.c[0][1] * dL_da + (T.c[0][1] * T.c[1][2] + T.c[0][2] * T.c[1][1]) * dL_db +
-                2 * T.c[1][1] * T.c[1][2] * dL_dc;
-    }
-    const float dL_dT00 = 2 * (T.c[0][0] * Vrk.c[0][0] + T.c[0][1] * Vrk.c[0][1] + T.c[0][2] * Vrk.c[0][2]) * dL_da +
-                          (T.c[1][0] * Vrk.c[0][0] + T.c[1][1] * Vrk.c[0][1] + T.c[1][2] * Vrk.c[0][2]) * dL_db;
-    const float dL_dT01 = 2 * (T.c[0][0] * Vrk.c[1][0] + T.c[0][1] * Vrk.c[1][1] + T.c[0][2] * Vrk.c[1][2]) * dL_da +
-                          (T.c[1][0] * Vrk.c[1][0] + T.c[1][1] * Vrk.c[1][1] + T.c[1][2] * Vrk.c[1][2]) * dL_db;
-    const float dL_dT02 = 2 * (T.c[0][0] * Vrk.c[2][0] + T.c[0][1] * Vrk.c[2][1] + T.c[0][2] * Vrk.c[2][2]) * dL_da +
-                          (T.c[1][0] * Vrk.c[2][0] + T.c[1][1] * Vrk.c[2][1] + T.c[1][2] * Vrk.c[2][2]) * dL_db;
-    const float dL_dT10 = 2 * (T.c[1][0] * Vrk.c[0][0] + T.c[1][1] * Vrk.c[0][1] + T.c[1][2] * Vrk.c[0][2]) * dL_dc +
-                          (T.c[0][0] * Vrk.c[0][0] + T.c[0][1] * Vrk.c[0][1] + T.c[0][2] * Vrk.c[0][2]) * dL_db;
-    const float dL_dT11 = 2 * (T.c[1][0] * Vrk.c[1][0] + T.c[1][1] * Vrk.c[1][1] + T.c[1][2] * Vrk.c[1][2]) * dL_dc +
-                          (T.c[0][0] * Vrk.c[1][0] + T.c[0][1] * Vrk.c[1][1] + T.c[0][2] * Vrk.c[1][2]) * dL_db;
-    const float dL_dT12 = 2 * (T.c[1][0] * Vrk.c[2][0] + T.c[1][1] * Vrk.c[2][1] + T.c[1][2] * Vrk.c[2][2]) * dL_dc +
-                          (T.c[0][0] * Vrk.c[2][0] + T.c[0][1] * Vrk.c[2][1] + T.c[0][2] * Vrk.c[2][2]) * dL_db;
-    const Mat3& Wm = fr.W;
-    const float dL_dJ00 = Wm.c[0][0] * dL_dT00 + Wm.c[0][1] * dL_dT01 + Wm.c[0][2] * dL_dT02;
-    const float dL_dJ02 = Wm.c[2][0] * dL_dT00 + Wm.c[2][1] * dL_dT01 + Wm.c[2][2] * dL_dT02;
-    const float dL_dJ11 = Wm.c[1][0] * dL_dT10 + Wm.c[1][1] * dL_dT11 + Wm.c[1][2] * dL_dT12;
-    const float dL_dJ12 = Wm.c[2][0] * dL_dT10 + Wm.c[2][1] * dL_dT11 + Wm.c[2][2] * dL_dT12;
-    const float tz = 1.f / fr.t.z;
-    const float tz2 = tz * tz;
-    const float tz3 = tz2 * tz;
-    const float dL_dtx = x_grad_mul * -focal_x * tz2 * dL_dJ02;
-    const float dL_dty = y_grad_mul * -focal_y * tz2 * dL_dJ12;
-    const float dL_dtz = -focal_x * tz2 * dL_dJ00 - focal_y * tz2 * dL_dJ11 + (2 * focal_x * fr.t.x) * tz3 * dL_dJ02 +
-                         (2 * focal_y * fr.t.y) * tz3 * dL_dJ12;
-    dmean = xform_vec4x3_T(make_float3(dL_dtx, dL_dty, dL_dtz), view);
 
-    // ---------------- screen-space mean -> 3D mean (backward.cu:366-381)
-    const float4 m_hom = xform4x4(mean, proj);
-    const float m_w = 1.0f / (m_hom.w + 0.0000001f);
-    const float mul1 = (proj[0] * mean.x + proj[4] * mean.y + proj[8] * mean.z + proj[12]) * m_w * m_w;
-    const float mul2 = (proj[1] * mean.x + proj[5] * mean.y + proj[9] * mean.z + proj[13]) * m_w * m_w;
-    float3 dm;
-    dm.x = (proj[0] * m_w - proj[3] * mul1) * dm2.x + (proj[1] * m_w - proj[3] * mul2) * dm2.y;
-    dm.y = (proj[4] * m_w - proj[7] * mul1) * dm2.x + (proj[5] * m_w - proj[7] * mul2) * dm2.y;
-    dm.z = (proj[8] * m_w - proj[11] * mul1) * dm2.x + (proj[9] * m_w - proj[11] * mul2) * dm2.y;
-    dmean.x += dm.x;
-    dmean.y += dm.y;
-    dmean.z += dm.z;
-
-    // ---------------- SH colour (backward.cu:20-139, 383-385)
-    if (shs) {
-      const float3 cp = make_float3(cam_pos[0], cam_pos[1], cam_pos[2]);
-      float sh[48], dsh[48];
-      load_sh(shs, idx, M, (D + 1) * (D + 1), sh);
-      const float3 dms = sh_backward(D, mean, cp, sh, g.clamped + 3 * idx, dcol, dsh);
-      dmean.x += dms.x;
-      dmean.y += dms.y;
-      dmean.z += dms.z;
-      float* dst = dL_dsh + (size_t)idx * M * 3;
-      if (M == 16) {
+      float dcov[6] = {0, 0, 0, 0, 0, 0};
+      float3 dmean = make_float3(0, 0, 0);
+      float3 dscale = make_float3(0, 0, 0);
+      float4 drot = make_float4(0, 0, 0, 0);
+      float w[16], dRGB[3] = {0.f, 0.f, 0.f};
 #pragma unroll
-        for (int i = 0; i < 12; ++i) {
-          float4 o = make_float4(dsh[4 * i], dsh[4 * i + 1], dsh[4 * i + 2], dsh[4 * i + 3]);
-          if (accumulate & ACC_COLOR) {
-            const float4 old = reinterpret_cast<float4*>(dst)[i];
-            o.x += old.x, o.y += old.y, o.z += old.z, o.w += old.w;
-          }
-          reinterpret_cast<float4*>(dst)[i] = o;
+      for (int k = 0; k < 16; ++k) w[k] = 0.f;
+      if (visible) {  // a culled Gaussian's gradients are zero
+        const float* mp = slab(means3D, DGR_PF_MEANS, 3) + 3 * g;
+        const float3 mean = make_float3(mp[0], mp[1], mp[2]);
+        const float* cov3D = cov3D_precomp ? slab(cov3D_precomp, DGR_PF_COV, 6) + 6 * g : gw.cov3D + 6 * g;
+        const float* view = views + 16 * f;
+        const float* proj = projs + 16 * f;
+        const float focal_x = cams.fx[f], focal_y = cams.fy[f], tan_fovx = cams.tanx[f], tan_fovy = cams.tany[f];
+        // ---------------- gradient through the 2D covariance / conic (backward.cu:144-274)
+        EwaFrame fr;
+        ewa_frame(mean, focal_x, focal_y, tan_fovx, tan_fovy, cov3D, view, fr);
+        const float limx = 1.3f * tan_fovx, limy = 1.3f * tan_fovy;
+        const float x_grad_mul = fr.txtz < -limx || fr.txtz > limx ? 0 : 1;
+        const float y_grad_mul = fr.tytz < -limy || fr.tytz > limy ? 0 : 1;
+        const float3 c2 = ewa_cov2d(fr);
+        const float a = c2.x, b = c2.y, c = c2.z;
+        const float denom = a * c - b * b;
+        float dL_da = 0, dL_db = 0, dL_dc = 0;
+        const float denom2inv = 1.0f / ((denom * denom) + 0.0000001f);
+        const Mat3& T = fr.T;
+        const Mat3& Vrk = fr.Vrk;
+        if (denom2inv != 0) {
+          dL_da = denom2inv * (-c * c * dcon.x + 2 * b * c * dcon.y + (denom - a * c) * dcon.z);
+          dL_dc = denom2inv * (-a * a * dcon.z + 2 * a * b * dcon.y + (denom - a * c) * dcon.x);
+          dL_db = denom2inv * 2 * (b * c * dcon.x - (denom + 2 * b * b) * dcon.y + a * b * dcon.z);
+          dcov[0] = (T.c[0][0] * T.c[0][0] * dL_da + T.c[0][0] * T.c[1][0] * dL_db + T.c[1][0] * T.c[1][0] * dL_dc);
+          dcov[3] = (T.c[0][1] * T.c[0][1] * dL_da + T.c[0][1] * T.c[1][1] * dL_db + T.c[1][1] * T.c[1][1] * dL_dc);
+          dcov[5] = (T.c[0][2] * T.c[0][2] * dL_da + T.c[0][2] * T.c[1][2] * dL_db + T.c[1][2] * T.c[1][2] * dL_dc);
+          dcov[1] = 2 * T.c[0][0] * T.c[0][1] * dL_da + (T.c[0][0] * T.c[1][1] + T.c[0][1] * T.c[1][0]) * dL_db +
+                    2 * T.c[1][0] * T.c[1][1] * dL_dc;
+          dcov[2] = 2 * T.c[0][0] * T.c[0][2] * dL_da + (T.c[0][0] * T.c[1][2] + T.c[0][2] * T.c[1][0]) * dL_db +
+                    2 * T.c[1][0] * T.c[1][2] * dL_dc;
+          dcov[4] = 2 * T.c[0][2] * T.c[0][1] * dL_da + (T.c[0][1] * T.c[1][2] + T.c[0][2] * T.c[1][1]) * dL_db +
+                    2 * T.c[1][1] * T.c[1][2] * dL_dc;
         }
-      } else {
+        const float dL_dT00 = 2 * (T.c[0][0] * Vrk.c[0][0] + T.c[0][1] * Vrk.c[0][1] + T.c[0][2] * Vrk.c[0][2]) * dL_da +
+                              (T.c[1][0] * Vrk.c[0][0] + T.c[1][1] * Vrk.c[0][1] + T.c[1][2] * Vrk.c[0][2]) * dL_db;
+        const float dL_dT01 = 2 * (T.c[0][0] * Vrk.c[1][0] + T.c[0][1] * Vrk.c[1][1] + T.c[0][2] * Vrk.c[1][2]) * dL_da +
+                              (T.c[1][0] * Vrk.c[1][0] + T.c[1][1] * Vrk.c[1][1] + T.c[1][2] * Vrk.c[1][2]) * dL_db;
+        const float dL_dT02 = 2 * (T.c[0][0] * Vrk.c[2][0] + T.c[0][1] * Vrk.c[2][1] + T.c[0][2] * Vrk.c[2][2]) * dL_da +
+                              (T.c[1][0] * Vrk.c[2][0] + T.c[1][1] * Vrk.c[2][1] + T.c[1][2] * Vrk.c[2][2]) * dL_db;
+        const float dL_dT10 = 2 * (T.c[1][0] * Vrk.c[0][0] + T.c[1][1] * Vrk.c[0][1] + T.c[1][2] * Vrk.c[0][2]) * dL_dc +
+                              (T.c[0][0] * Vrk.c[0][0] + T.c[0][1] * Vrk.c[0][1] + T.c[0][2] * Vrk.c[0][2]) * dL_db;
+        const float dL_dT11 = 2 * (T.c[1][0] * Vrk.c[1][0] + T.c[1][1] * Vrk.c[1][1] + T.c[1][2] * Vrk.c[1][2]) * dL_dc +
+                              (T.c[0][0] * Vrk.c[1][0] + T.c[0][1] * Vrk.c[1][1] + T.c[0][2] * Vrk.c[1][2]) * dL_db;
+        const float dL_dT12 = 2 * (T.c[1][0] * Vrk.c[2][0] + T.c[1][1] * Vrk.c[2][1] + T.c[1][2] * Vrk.c[2][2]) * dL_dc +
+                              (T.c[0][0] * Vrk.c[2][0] + T.c[0][1] * Vrk.c[2][1] + T.c[0][2] * Vrk.c[2][2]) * dL_db;
+        const Mat3& Wm = fr.W;
+        const float dL_dJ00 = Wm.c[0][0] * dL_dT00 + Wm.c[0][1] * dL_dT01 + Wm.c[0][2] * dL_dT02;
+        const float dL_dJ02 = Wm.c[2][0] * dL_dT00 + Wm.c[2][1] * dL_dT01 + Wm.c[2][2] * dL_dT02;
+        const float dL_dJ11 = Wm.c[1][0] * dL_dT10 + Wm.c[1][1] * dL_dT11 + Wm.c[1][2] * dL_dT12;
+        const float dL_dJ12 = Wm.c[2][0] * dL_dT10 + Wm.c[2][1] * dL_dT11 + Wm.c[2][2] * dL_dT12;
+        const float tz = 1.f / fr.t.z;
+        const float tz2 = tz * tz;
+        const float tz3 = tz2 * tz;
+        const float dL_dtx = x_grad_mul * -focal_x * tz2 * dL_dJ02;
+        const float dL_dty = y_grad_mul * -focal_y * tz2 * dL_dJ12;
+        const float dL_dtz = -focal_x * tz2 * dL_dJ00 - focal_y * tz2 * dL_dJ11 + (2 * focal_x * fr.t.x) * tz3 * dL_dJ02 +
+                             (2 * focal_y * fr.t.y) * tz3 * dL_dJ12;
+        dmean = xform_vec4x3_T(make_float3(dL_dtx, dL_dty, dL_dtz), view);
+
+        // ---------------- screen-space mean -> 3D mean (backward.cu:366-381)
+        const float4 m_hom = xform4x4(mean, proj);
+        const float m_w = 1.0f / (m_hom.w + 0.0000001f);
+        const float mul1 = (proj[0] * mean.x + proj[4] * mean.y + proj[8] * mean.z + proj[12]) * m_w * m_w;
+        const float mul2 = (proj[1] * mean.x + proj[5] * mean.y + proj[9] * mean.z + proj[13]) * m_w * m_w;
+        float3 dm;
+        dm.x = (proj[0] * m_w - proj[3] * mul1) * dm2.x + (proj[1] * m_w - proj[3] * mul2) * dm2.y;
+        dm.y = (proj[4] * m_w - proj[7] * mul1) * dm2.x + (proj[5] * m_w - proj[7] * mul2) * dm2.y;
+        dm.z = (proj[8] * m_w - proj[11] * mul1) * dm2.x + (proj[9] * m_w - proj[11] * mul2) * dm2.y;
+        dmean.x += dm.x;
+        dmean.y += dm.y;
+        dmean.z += dm.z;
+
+
+        // ---------------- SH colour (backward.cu:20-139, 383-385)
+        if (shs) {
+          const float3 cp = make_float3(cam_poses[3 * f], cam_poses[3 * f + 1], cam_poses[3 * f + 2]);
+          float sh[48];
+          load_sh(slab(shs, DGR_PF_COLOR, M * 3), g, M, ncoef, sh);
+          const float3 dms = sh_backward(D, mean, cp, sh, gw.clamped + 3 * g, dcol, w, dRGB);
+          dmean.x += dms.x;
+          dmean.y += dms.y;
+          dmean.z += dms.z;
+        }
+        const float* sc_f = scales ? slab(scales, DGR_PF_SCALES, 3) : nullptr;
+        const float* rot_f = rotations ? slab(rotations, DGR_PF_ROTS, 4) : nullptr;
+        // ---------------- 3D covariance -> scale / rotation (backward.cu:279-341)
+        if (sc_f) {
+          const float3 sc = make_float3(sc_f[3 * g], sc_f[3 * g + 1], sc_f[3 * g + 2]);
+          const float4 q = __ldg(reinterpret_cast<const float4*>(rot_f) + g);
+          const float r = q.x, x = q.y, y = q.z, z = q.w;
+          Mat3 R;
+          quat_to_R(q, R);
+          const float3 s = make_float3(scale_modifier * sc.x, scale_modifier * sc.y, scale_modifier * sc.z);
+          Mat3 S;
 #pragma unroll
-        for (int i = 0; i < 48; ++i)
-          if (i < M * 3) acc_store(&dst[i], dsh[i], accumulate & ACC_COLOR);
+          for (int i = 0; i < 3; ++i)
+#pragma unroll
+            for (int j = 0; j < 3; ++j) S.c[i][j] = (i == j) ? 1.0f : 0.0f;
+          S.c[0][0] = s.x;
+          S.c[1][1] = s.y;
+          S.c[2][2] = s.z;
+          const Mat3 Mm = mat3_mul(S, R);
+          Mat3 dSig;
+          dSig.c[0][0] = dcov[0];
+          dSig.c[0][1] = 0.5f * dcov[1];
+          dSig.c[0][2] = 0.5f * dcov[2];
+          dSig.c[1][0] = 0.5f * dcov[1];
+          dSig.c[1][1] = dcov[3];
+          dSig.c[1][2] = 0.5f * dcov[4];
+          dSig.c[2][0] = 0.5f * dcov[2];
+          dSig.c[2][1] = 0.5f * dcov[4];
+          dSig.c[2][2] = dcov[5];
+          Mat3 M2;
+#pragma unroll
+          for (int i = 0; i < 3; ++i)
+#pragma unroll
+            for (int j = 0; j < 3; ++j) M2.c[i][j] = 2.0f * Mm.c[i][j];
+          const Mat3 dL_dM = mat3_mul(M2, dSig);
+          const Mat3 Rt = mat3_T(R);
+          Mat3 dMt = mat3_T(dL_dM);
+          dscale.x = Rt.c[0][0] * dMt.c[0][0] + Rt.c[0][1] * dMt.c[0][1] + Rt.c[0][2] * dMt.c[0][2];
+          dscale.y = Rt.c[1][0] * dMt.c[1][0] + Rt.c[1][1] * dMt.c[1][1] + Rt.c[1][2] * dMt.c[1][2];
+          dscale.z = Rt.c[2][0] * dMt.c[2][0] + Rt.c[2][1] * dMt.c[2][1] + Rt.c[2][2] * dMt.c[2][2];
+#pragma unroll
+          for (int j = 0; j < 3; ++j) {
+            dMt.c[0][j] *= s.x;
+            dMt.c[1][j] *= s.y;
+            dMt.c[2][j] *= s.z;
+          }
+          drot.x = 2 * z * (dMt.c[0][1] - dMt.c[1][0]) + 2 * y * (dMt.c[2][0] - dMt.c[0][2]) +
+                   2 * x * (dMt.c[1][2] - dMt.c[2][1]);
+          drot.y = 2 * y * (dMt.c[1][0] + dMt.c[0][1]) + 2 * z * (dMt.c[2][0] + dMt.c[0][2]) +
+                   2 * r * (dMt.c[1][2] - dMt.c[2][1]) - 4 * x * (dMt.c[2][2] + dMt.c[1][1]);
+          drot.z = 2 * x * (dMt.c[1][0] + dMt.c[0][1]) + 2 * r * (dMt.c[2][0] - dMt.c[0][2]) +
+                   2 * z * (dMt.c[1][2] + dMt.c[2][1]) - 4 * y * (dMt.c[2][2] + dMt.c[0][0]);
+          drot.w = 2 * r * (dMt.c[0][1] - dMt.c[1][0]) + 2 * x * (dMt.c[2][0] + dMt.c[0][2]) +
+                   2 * y * (dMt.c[1][2] + dMt.c[2][1]) - 4 * z * (dMt.c[1][1] + dMt.c[0][0]);
+        }
+      }
+      if (sum_sh) {
+#pragma unroll
+        for (int k = 0; k < 16; ++k) put(true, nullptr, 0, SL_W, k, w[k]);
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) put(true, nullptr, 0, SL_RGB, ch, dRGB[ch]);
+      } else if (shs) {
+        float* dst = dL_dsh + fg * M * 3;
+        if (M == 16) {
+#pragma unroll
+          for (int i = 0; i < 12; ++i) {
+            float o[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) o[j] = (4 * i + j) / 3 < ncoef ? w[(4 * i + j) / 3] * dRGB[(4 * i + j) % 3] : 0.f;
+            reinterpret_cast<float4*>(dst)[i] = make_float4(o[0], o[1], o[2], o[3]);
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < 48; ++i)
+            if (i < M * 3) dst[i] = i / 3 < ncoef ? w[i / 3] * dRGB[i % 3] : 0.f;
+        }
+      }
+      put(sum & DGR_PF_MEANS, dL_dmean3D, 3, SL_MEAN, 0, dmean.x);
+      put(sum & DGR_PF_MEANS, dL_dmean3D, 3, SL_MEAN, 1, dmean.y);
+      put(sum & DGR_PF_MEANS, dL_dmean3D, 3, SL_MEAN, 2, dmean.z);
+      if (dL_dcov3D) {
+#pragma unroll
+        for (int k = 0; k < 6; ++k) put(sum & DGR_PF_COV, dL_dcov3D, 6, SL_COV, k, dcov[k]);
+      }
+      put(sum & DGR_PF_SCALES, dL_dscale, 3, SL_SCALE, 0, dscale.x);
+      put(sum & DGR_PF_SCALES, dL_dscale, 3, SL_SCALE, 1, dscale.y);
+      put(sum & DGR_PF_SCALES, dL_dscale, 3, SL_SCALE, 2, dscale.z);
+      put(sum & DGR_PF_ROTS, dL_drot, 4, SL_ROT, 0, drot.x);
+      put(sum & DGR_PF_ROTS, dL_drot, 4, SL_ROT, 1, drot.y);
+      put(sum & DGR_PF_ROTS, dL_drot, 4, SL_ROT, 2, drot.z);
+      put(sum & DGR_PF_ROTS, dL_drot, 4, SL_ROT, 3, drot.w);
+    }
+    if (!sum && !sum_col) continue;  // uniform: nothing is summed over the frames
+    __syncthreads();
+    // ---- sum this pass's frames into the block's rows of each summed output: row q, column c is
+    // element e = q * width + c of the block's slice (the warp stores 128 consecutive bytes); a pass after
+    // the first continues from the value the previous pass stored
+    const int nf = min(FB, F - f0), nval = min(NG, P - g0);
+    auto sum_frames = [&](float* out, int width, int slot) {
+      float* dst = out + (size_t)g0 * width;
+      for (int e = tid; e < nval * width; e += NT) {
+        const int q = e / width;
+        const float* s = s_stage + (slot + e - q * width) * PB_STRIDE + q;
+        float acc = f0 ? dst[e] : s[0];
+        for (int i = f0 ? 0 : 1; i < nf; ++i) acc = acc + s[i * NG];
+        dst[e] = acc;
+      }
+    };
+    if (sum & DGR_PF_OPAC) sum_frames(dL_dopacity, 1, SL_OPAC);
+    if (sum_col) sum_frames(dL_dcolor, 3, SL_COL);
+    if (sum & DGR_PF_MEANS) sum_frames(dL_dmean3D, 3, SL_MEAN);
+    if ((sum & DGR_PF_COV) && dL_dcov3D) sum_frames(dL_dcov3D, 6, SL_COV);
+    if (sum & DGR_PF_SCALES) sum_frames(dL_dscale, 3, SL_SCALE);
+    if (sum & DGR_PF_ROTS) sum_frames(dL_drot, 4, SL_ROT);
+    if (sum_sh) {  // dL_dsh[k][ch] = sum over frames of w[k] dRGB[ch], each product rounded before it is added
+      const int width = 3 * M;
+      float* dst = dL_dsh + (size_t)g0 * width;
+      for (int e = tid; e < nval * width; e += NT) {
+        const int q = e / width, c = e - q * width, k = c / 3;
+        const float* sw = s_stage + (SL_W + k) * PB_STRIDE + q;
+        const float* sd = s_stage + (SL_RGB + c - 3 * k) * PB_STRIDE + q;
+        float acc = 0.f;
+        if (k < ncoef) {
+          acc = f0 ? dst[e] : __fmul_rn(sw[0], sd[0]);
+          for (int i = f0 ? 0 : 1; i < nf; ++i) acc = __fadd_rn(acc, __fmul_rn(sw[i * NG], sd[i * NG]));
+        }
+        dst[e] = acc;
       }
     }
-    // ---------------- 3D covariance -> scale / rotation (backward.cu:279-341)
-    if (scales) {
-      const float3 sc = make_float3(scales[3 * idx], scales[3 * idx + 1], scales[3 * idx + 2]);
-      const float4 q = __ldg(reinterpret_cast<const float4*>(rotations) + idx);
-      const float r = q.x, x = q.y, y = q.z, z = q.w;
-      Mat3 R;
-      quat_to_R(q, R);
-      const float3 s = make_float3(scale_modifier * sc.x, scale_modifier * sc.y, scale_modifier * sc.z);
-      Mat3 S;
-#pragma unroll
-      for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) S.c[i][j] = (i == j) ? 1.0f : 0.0f;
-      S.c[0][0] = s.x;
-      S.c[1][1] = s.y;
-      S.c[2][2] = s.z;
-      const Mat3 Mm = mat3_mul(S, R);
-      Mat3 dSig;
-      dSig.c[0][0] = dcov[0];
-      dSig.c[0][1] = 0.5f * dcov[1];
-      dSig.c[0][2] = 0.5f * dcov[2];
-      dSig.c[1][0] = 0.5f * dcov[1];
-      dSig.c[1][1] = dcov[3];
-      dSig.c[1][2] = 0.5f * dcov[4];
-      dSig.c[2][0] = 0.5f * dcov[2];
-      dSig.c[2][1] = 0.5f * dcov[4];
-      dSig.c[2][2] = dcov[5];
-      Mat3 M2;
-#pragma unroll
-      for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) M2.c[i][j] = 2.0f * Mm.c[i][j];
-      const Mat3 dL_dM = mat3_mul(M2, dSig);
-      const Mat3 Rt = mat3_T(R);
-      Mat3 dMt = mat3_T(dL_dM);
-      dscale.x = Rt.c[0][0] * dMt.c[0][0] + Rt.c[0][1] * dMt.c[0][1] + Rt.c[0][2] * dMt.c[0][2];
-      dscale.y = Rt.c[1][0] * dMt.c[1][0] + Rt.c[1][1] * dMt.c[1][1] + Rt.c[1][2] * dMt.c[1][2];
-      dscale.z = Rt.c[2][0] * dMt.c[2][0] + Rt.c[2][1] * dMt.c[2][1] + Rt.c[2][2] * dMt.c[2][2];
-#pragma unroll
-      for (int j = 0; j < 3; ++j) {
-        dMt.c[0][j] *= s.x;
-        dMt.c[1][j] *= s.y;
-        dMt.c[2][j] *= s.z;
-      }
-      drot.x = 2 * z * (dMt.c[0][1] - dMt.c[1][0]) + 2 * y * (dMt.c[2][0] - dMt.c[0][2]) +
-               2 * x * (dMt.c[1][2] - dMt.c[2][1]);
-      drot.y = 2 * y * (dMt.c[1][0] + dMt.c[0][1]) + 2 * z * (dMt.c[2][0] + dMt.c[0][2]) +
-               2 * r * (dMt.c[1][2] - dMt.c[2][1]) - 4 * x * (dMt.c[2][2] + dMt.c[1][1]);
-      drot.z = 2 * x * (dMt.c[1][0] + dMt.c[0][1]) + 2 * r * (dMt.c[2][0] - dMt.c[0][2]) +
-               2 * z * (dMt.c[1][2] + dMt.c[2][1]) - 4 * y * (dMt.c[2][2] + dMt.c[0][0]);
-      drot.w = 2 * r * (dMt.c[0][1] - dMt.c[1][0]) + 2 * x * (dMt.c[2][0] + dMt.c[0][2]) +
-               2 * y * (dMt.c[1][2] + dMt.c[2][1]) - 4 * z * (dMt.c[1][1] + dMt.c[0][0]);
-    }
-  }
-  acc_store(&dL_dmean3D[3 * idx + 0], dmean.x, accumulate & ACC_MEANS);
-  acc_store(&dL_dmean3D[3 * idx + 1], dmean.y, accumulate & ACC_MEANS);
-  acc_store(&dL_dmean3D[3 * idx + 2], dmean.z, accumulate & ACC_MEANS);
-#pragma unroll
-  for (int k = 0; k < 6; ++k) acc_store(&dL_dcov3D[6 * idx + k], dcov[k], accumulate & ACC_COV);
-  acc_store(&dL_dscale[3 * idx + 0], dscale.x, accumulate & ACC_SCALES);
-  acc_store(&dL_dscale[3 * idx + 1], dscale.y, accumulate & ACC_SCALES);
-  acc_store(&dL_dscale[3 * idx + 2], dscale.z, accumulate & ACC_SCALES);
-  {
-    float4 o = drot;
-    if (accumulate & ACC_ROTS) {
-      const float4 old = reinterpret_cast<float4*>(dL_drot)[idx];
-      o.x += old.x, o.y += old.y, o.z += old.z, o.w += old.w;
-    }
-    reinterpret_cast<float4*>(dL_drot)[idx] = o;
+    __syncthreads();  // the next pass overwrites the staging area
   }
 }
 
@@ -647,19 +725,25 @@ cudaError_t launch_render_bwd(const BwdArgs& a, cudaStream_t s) {
   return cudaGetLastError();
 }
 
-// chain rule from the moments to the inputs (short); with a.accumulate it adds to the outputs, so
-// the calls of a frame batch must be ordered (same stream)
+// chain rule from the moments to the inputs, all frames of a batch in one launch (after every frame's
+// render_bwd_kernel)
 cudaError_t launch_preprocess_bwd(const BwdArgs& a, cudaStream_t s) {
   if (a.P == 0) return cudaSuccess;
-  GeomWS g = GeomWS::from((char*)a.geom_ws, a.P);
-  const float focal_y = a.H / (2.0f * a.tan_fovy);
-  const float focal_x = a.W / (2.0f * a.tan_fovx);
-  const int* radii = a.radii ? a.radii : g.radii;
+  if (a.F < 1 || a.F > PB_MAX_FRAMES) return cudaErrorInvalidValue;
+  PbCams c = {};
+  for (int f = 0; f < a.F; ++f) {
+    c.tanx[f] = a.tan_fovx[f];
+    c.tany[f] = a.tan_fovy[f];
+    c.fx[f] = a.W / (2.0f * a.tan_fovx[f]);
+    c.fy[f] = a.H / (2.0f * a.tan_fovy[f]);
+  }
+  const int nt = a.F == 1 ? 128 : 256, ng = nt / pb_frames_per_pass(a.F);
   g_prof.begin(6, s);
-  launch_pdl(preprocess_bwd_kernel, dim3((a.P + 127) / 128), dim3(128), 0, s, a.P, a.D, a.M, a.means3D, radii, a.shs,
-             a.scales, a.rotations, a.scale_modifier, a.cov3D_precomp, a.viewmatrix, a.projmatrix, focal_x, focal_y,
-             a.tan_fovx, a.tan_fovy, a.cam_pos, g, a.dL_dmean2D, a.dL_dconic, a.dL_dopacity, a.dL_dcolor, a.dL_dmean3D,
-             a.dL_dcov3D, a.dL_dsh, a.dL_dscale, a.dL_drot, a.accumulate);
+  launch_pdl(a.F == 1 ? preprocess_bwd_kernel<128, 3> : preprocess_bwd_kernel<256, 2>, dim3((a.P + ng - 1) / ng),
+             dim3(nt), 0, s, a.F, a.P, a.D, a.M, a.per_frame, a.means3D, a.radii, a.shs, a.scales, a.rotations,
+             a.scale_modifier, a.cov3D_precomp, a.viewmatrix, a.projmatrix, a.cam_pos, c, (char*)a.geom_ws,
+             a.geom_stride, a.dL_dmean2D, a.dL_dconic, a.dL_dopacity, a.dL_dcolor, a.dL_dmean3D, a.dL_dcov3D,
+             a.dL_dsh, a.dL_dscale, a.dL_drot);
   g_prof.end(6, s);
   return cudaGetLastError();
 }

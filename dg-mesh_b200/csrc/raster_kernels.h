@@ -35,15 +35,21 @@ struct BwdArgs {
   const float *means3D, *shs, *colors_precomp, *scales;
   float scale_modifier;
   const float *rotations, *cov3D_precomp, *viewmatrix, *projmatrix, *cam_pos;
-  float tan_fovx, tan_fovy;
+  const float *tan_fovx, *tan_fovy;  // host arrays, one value per frame
   const int* radii;
   void *geom_ws, *binning_ws, *img_ws;
   int64_t R_cap;
   const float* dL_dpix;
   float *dL_dmean2D, *dL_dconic, *dL_dopacity, *dL_dcolor, *dL_dmean3D, *dL_dcov3D, *dL_dsh, *dL_dscale, *dL_drot;
-  int accumulate;  // bit mask DGR_PF_*: outputs that are ADDED to what the buffers hold (shared inputs of a
-                   // frame batch, frames after the first); 0: every parameter gradient is written
+  // launch_preprocess_bwd covers F frames (1 <= F <= PB_MAX_FRAMES) in one launch: frame f reads the camera at
+  // index f (viewmatrix + 16 f, ..., tan_fovx[f]), its workspace at geom_ws + f * geom_stride, radii + f * P,
+  // and the slab f of each input whose DGR_PF_* bit is set in per_frame.  dL_dmean2D (and dL_dconic) are
+  // [F,P,.]; every other gradient is [F,P,.] when its bit is set and the sum over the frames otherwise.
+  // launch_render_bwd reads one frame: frame 0 of the above.
+  int F, per_frame;
+  size_t geom_stride;
 };
+#define PB_MAX_FRAMES 64
 
 // event pairs around kernels (see dgm_profile_enable in include/dgmesh_b200.h)
 struct Profiler {
@@ -74,7 +80,6 @@ extern Profiler g_prof;
 
 cudaError_t launch_forward(const FwdArgs& a, cudaStream_t s);
 cudaError_t launch_backward(const BwdArgs& a, cudaStream_t s);
-// same, with an event to wait on before / to record after the (accumulating) per-Gaussian kernel
 cudaError_t launch_binning(const FwdArgs& a, cudaStream_t s);
 cudaError_t launch_render(const FwdArgs& a, cudaStream_t s);
 cudaError_t launch_render_bwd(const BwdArgs& a, cudaStream_t s);

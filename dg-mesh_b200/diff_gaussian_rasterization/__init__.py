@@ -441,9 +441,11 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
         def nf(bit):
             return F if (pf & bit) else 1
 
-        # m2d[F,P,3] opac col m3d cov scale rot sh -- per-frame inputs get F slabs
-        widths = (3 * F, nf(_PF_OPAC), 3 * (nf(_PF_COLOR) if sh is None else 1), 3 * nf(_PF_MEANS),
-                  6 * nf(_PF_COV), 3 * nf(_PF_SCALES), 4 * nf(_PF_ROTS), 3 * M * nf(_PF_COLOR))
+        # m2d[F,P,3] opac col m3d cov scale rot sh -- per-frame inputs get F slabs; the colour gradient (with SH
+        # colours) and the cov3D gradient (without cov3D_precomp) are not returned, so they are not computed
+        widths = (3 * F, nf(_PF_OPAC), 3 * nf(_PF_COLOR) if col is not None else 0, 3 * nf(_PF_MEANS),
+                  6 * nf(_PF_COV) if cov is not None else 0, 3 * nf(_PF_SCALES), 4 * nf(_PF_ROTS),
+                  3 * M * nf(_PF_COLOR))
         offs, o = [], 0
         for w in widths:
             offs.append(o)
@@ -466,8 +468,9 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
         rc = _dgm_lib.lib().dgr_backward_batch(
             F, P, rs0.sh_degree, M, p(bg), W, H, p(means3D), p(sh), p(col), p(sc), float(rs0.scale_modifier), p(rot),
             p(cov), pf, p(views), p(projs), p(cams), tx, ty, p(radii), ws.geom, ws.gs, ws.binning, ws.bs, ws.R_cap,
-            ws.img, ws.is_, p(dpix), ptrs[0], ptrs[1], ptrs[2], ptrs[3], ptrs[4], ptrs[7] if M else None, ptrs[5],
-            ptrs[6], _N_STREAMS, _dgm_lib.stream_ptr())
+            ws.img, ws.is_, p(dpix), ptrs[0], ptrs[1], ptrs[2] if col is not None else None, ptrs[3],
+            ptrs[4] if cov is not None else None, ptrs[7] if M else None, ptrs[5], ptrs[6], _N_STREAMS,
+            _dgm_lib.stream_ptr())
         _dgm_lib.check(rc, "dgr_backward_batch")
         return (gview(3, _PF_MEANS, P, 3), gview(0, 0, F, P, 3) if ctx.has_m2d else None,
                 gview(7, _PF_COLOR, P, M, 3) if sh is not None else None,

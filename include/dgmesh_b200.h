@@ -154,7 +154,11 @@ int dgr_backward(int P, int D, int M,
  *                      reported by dgr_workspace_sizes, multiple of 128)
  * backward: dL_dpix[F,3,H,W] -> dL_dmean2D[F,P,3] per frame; dL_dopacity[P], dL_dcolor[P,3],
  * dL_dmean3D[P,3], dL_dcov3D[P,6], dL_dsh[P,M,3], dL_dscale[P,3], dL_drot[P,4] summed over
- * frames (fully written, no zero-fill needed).  n_streams: 1..4 side streams.
+ * frames in frame order (fully written, no zero-fill needed).  With shs, dL_dcolor is [P,3] summed
+ * over the frames whatever the mask, and may be NULL; without cov3D_precomp, dL_dcov3D may be NULL.
+ * Both are intermediate gradients that only a caller inspecting them needs.  The per-Gaussian part
+ * of the backward runs once for all frames after every frame's blend backward; at most 64 frames.
+ * n_streams: 1..4 side streams.
  * ------------------------------------------------------------------------ */
 #define DGR_PF_MEANS 1
 #define DGR_PF_SCALES 2

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Where does a frame batch spend its time?  Times the forward and backward halves of the bench's
-8-frame batch separately (CUDA events, synchronised between the halves) next to the sum of the
-stand-alone kernel durations."""
+"""Where does a frame batch spend its time?  Times the forward and backward halves of the bench's headline
+step (the 8-frame dynamic batch: per-frame deformed means / scales / rotations, shared opacity and SH)
+separately, with CUDA events and a synchronise between the halves."""
 import os
 import sys
 
@@ -14,7 +14,8 @@ import diff_gaussian_rasterization as dgr  # noqa: E402
 
 dev = torch.device("cuda")
 sc, cams, dpix = bench.make_inputs(dev)
-leaves, gflat = bench.flat_params(sc, dev)
+deltas = bench.make_deltas(sc, dev)
+leaves, gflat, _ = bench.flat_params(sc, dev)
 bg = torch.ones(3, device=dev)
 frames = list(range(bench.FRAMES))
 settings = bench.batch_settings(dgr, cams, bg, frames)
@@ -25,23 +26,28 @@ def ev():
     return torch.cuda.Event(enable_timing=True)
 
 
-fw, bw, tot = [], [], []
-for it in range(12):
+fw, bw = [], []
+for it in range(24):
     gflat.zero_()
     torch.cuda.synchronize()
-    e0, e1, e2 = ev(), ev(), ev()
+    e0, e1 = ev(), ev()
     e0.record()
     color, radii = dgr.BatchGaussianRasterizer(settings)(
-        means3D=leaves["means3D"], means2D=None, opacities=leaves["opacities"], shs=leaves["shs"],
-        scales=leaves["scales"], rotations=leaves["rotations"])
+        means3D=leaves["means3D"][None] + deltas["means3D"], means2D=None, opacities=leaves["opacities"],
+        shs=leaves["shs"], scales=leaves["scales"][None] + deltas["scales"],
+        rotations=leaves["rotations"][None] + deltas["rotations"])
     e1.record()
     torch.cuda.synchronize()
-    e1b = ev()
+    e1b, e2 = ev(), ev()
     e1b.record()
     color.backward(dp)
     e2.record()
     torch.cuda.synchronize()
     if it >= 4:
-        fw.append(e0.elapsed_time(e1)); bw.append(e1b.elapsed_time(e2))
-print(f"streams={os.environ.get('DGMESH_B200_STREAMS', 'default')}  forward {sum(fw)/len(fw):.3f} ms   backward {sum(bw)/len(bw):.3f} ms  "
-      f"(8 frames; stand-alone kernel sums: fwd 8x(0.115 binning + 0.096 blend), bwd 8x(0.198 + 0.027))")
+        fw.append(e0.elapsed_time(e1))
+        bw.append(e1b.elapsed_time(e2))
+fw.sort()
+bw.sort()
+print(f"streams={os.environ.get('DGMESH_B200_STREAMS', 'default')}  {bench.FRAMES} frames: "
+      f"forward median {fw[len(fw) // 2]:.3f} ms, backward median {bw[len(bw) // 2]:.3f} ms "
+      f"(min {bw[0]:.3f}, max {bw[-1]:.3f}) over {len(bw)} steps")

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Text timeline of one 8-frame batch (forward + backward): when each kernel of each frame reached the
+"""Text timeline of one step of the bench's 8-frame dynamic batch (forward + backward): when each kernel of each frame reached the
 front of its stream and when it finished (dgm_profile_enable(2); CUDA events on the internal streams)."""
 import ctypes
 import os
@@ -16,7 +16,8 @@ import diff_gaussian_rasterization as dgr  # noqa: E402
 NAMES = ["preprocess", "tile_scan", "scatter", "sort_pack", "render_fwd", "render_bwd", "preprocess_bwd", "count"]
 dev = torch.device("cuda")
 sc, cams, dpix = bench.make_inputs(dev)
-leaves, gflat = bench.flat_params(sc, dev)
+deltas = bench.make_deltas(sc, dev)
+leaves, gflat, _ = bench.flat_params(sc, dev)
 bg = torch.ones(3, device=dev)
 settings = bench.batch_settings(dgr, cams, bg, list(range(bench.FRAMES)))
 dp = torch.stack([d.to(dev) for d in dpix]).contiguous()
@@ -24,7 +25,7 @@ dp = torch.stack([d.to(dev) for d in dpix]).contiguous()
 
 def step():
     gflat.zero_()
-    bench.run_batch(dgr, leaves, settings, dp)
+    bench.run_batch(dgr, leaves, settings, dp, deltas=deltas)
 
 
 for _ in range(5):
