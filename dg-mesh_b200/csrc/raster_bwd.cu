@@ -408,13 +408,20 @@ __device__ __forceinline__ float3 sh_backward(int deg, const float3 pos, const f
 }
 
 // ---- per-Gaussian backward of a frame batch (F = 1: one frame).  A block covers NG Gaussians x FB frames per
-// pass (FB * NG = 256): warp w takes 32 consecutive Gaussians of frame f0 + w % FB, so per-frame slabs load
-// and store coalesced.  Gradients of per-frame inputs are written by the frame's thread.  Gradients of inputs
-// shared by the frames are staged per (frame, Gaussian) in shared memory and summed over the frames in frame
-// order f = 0, 1, ..., F - 1 (the rounding of F - 1 sequential fp32 additions), then written once per pass.
-// The SH gradient is staged as its two factors w[16], dRGB[3] and the products are formed by the summing
-// thread; for shared SH the coefficients of a Gaussian come from HBM once and from L1/L2 for the other frames.
-// staging slots: the SH factors w[16] and dRGB[3], opacity, colour, mean, scale, rotation, cov3D
+// pass (FB * NG = NT): warp w takes 32 consecutive Gaussians of frame f0 + w % FB, so per-frame slabs load
+// coalesced.  Every output is staged per (frame, Gaussian) in shared memory and written as rows of consecutive
+// floats (every store of a warp covers 128 consecutive bytes): gradients of per-frame inputs by the warp that
+// staged them, to the frame's slab; gradients of inputs shared by the frames by the whole block once per pass,
+// summed over the frames in frame order f = 0, 1, ..., F - 1 (the rounding of F - 1 sequential fp32
+// additions).  The SH gradient is staged as its two factors w[16], dRGB[3] and the products are formed by the
+// writing thread.
+//
+// The kernel streams about 220 B per (frame, Gaussian) against a few hundred flops, so it is bound by how many
+// bytes are in flight.  A thread therefore issues every load it needs at its top, before the visibility test,
+// which only selects the results (a culled Gaussian's gradients are zero).  With sh_smem the block's SH
+// coefficients (shared by the frames, 16 per Gaussian) arrive with one bulk copy issued at block start; it
+// overlaps the per-frame loads, and the frames' threads read them from shared memory.
+// staging slots: the SH factors w[16] and dRGB[3], opacity, colour, mean, scale, rotation, cov3D, 2D mean
 #define SL_W 0
 #define SL_RGB 16
 #define SL_OPAC 19
@@ -423,42 +430,62 @@ __device__ __forceinline__ float3 sh_backward(int deg, const float3 pos, const f
 #define SL_SCALE 26
 #define SL_ROT 29
 #define SL_COV 33
-#define SL_COUNT 39
+#define SL_M2D 39
+#define SL_COUNT 42
 
 // frames per pass of a 256-thread block (one frame: any block size)
 static __host__ __device__ inline int pb_frames_per_pass(int F) { return F >= 8 ? 8 : F >= 4 ? 4 : F >= 2 ? 2 : 1; }
+
+// dynamic shared memory of an NT-thread block: the block's SH coefficients (with sh_smem), then the staging area
+static inline size_t pb_smem_bytes(int NT, int F, int M, bool sh_smem) {
+  return (sh_smem ? (size_t)(NT / pb_frames_per_pass(F)) * M * 12 : 0) + (size_t)SL_COUNT * (NT + 1) * 4;
+}
 
 struct PbCams {  // per frame: tan(fov / 2) and focal lengths in pixels
   float tanx[PB_MAX_FRAMES], tany[PB_MAX_FRAMES], fx[PB_MAX_FRAMES], fy[PB_MAX_FRAMES];
 };
 
-// NT threads per block.  One frame (no staging) runs as 128-thread blocks, 3 per SM (the register budget of the
-// one-frame math without a cap); a batch as 256-thread blocks, 2 per SM, 128 registers, 8 frames per pass.
+// NT threads per block.  One frame runs as 128-thread blocks, 3 per SM (the register budget of the one-frame math
+// without a cap); a batch as 256-thread blocks, 2 per SM, 128 registers, 8 frames per pass.
+// sh_smem: M = 16 and shs is shared by the frames (or there is one frame).
 template <int NT, int MIN_BLOCKS>
 __global__ void __launch_bounds__(NT, MIN_BLOCKS) preprocess_bwd_kernel(
     int F, int P, int D, int M, int per_frame, const float* __restrict__ means3D, const int* __restrict__ radii,
-    const float* __restrict__ shs, const float* __restrict__ scales, const float* __restrict__ rotations,
-    float scale_modifier, const float* __restrict__ cov3D_precomp, const float* __restrict__ views,
-    const float* __restrict__ projs, const float* __restrict__ cam_poses, const PbCams cams, char* geom_ws,
-    size_t geom_stride, float* __restrict__ dL_dmean2D, float* __restrict__ dL_dconic,
-    float* __restrict__ dL_dopacity, float* __restrict__ dL_dcolor, float* __restrict__ dL_dmean3D,
-    float* __restrict__ dL_dcov3D, float* __restrict__ dL_dsh, float* __restrict__ dL_dscale,
-    float* __restrict__ dL_drot, int depth_grad) {
+    const float* __restrict__ shs, int sh_smem, const float* __restrict__ scales,
+    const float* __restrict__ rotations, float scale_modifier, const float* __restrict__ cov3D_precomp,
+    const float* __restrict__ views, const float* __restrict__ projs, const float* __restrict__ cam_poses,
+    const PbCams cams, char* geom_ws, size_t geom_stride, float* __restrict__ dL_dmean2D,
+    float* __restrict__ dL_dconic, float* __restrict__ dL_dopacity, float* __restrict__ dL_dcolor,
+    float* __restrict__ dL_dmean3D, float* __restrict__ dL_dcov3D, float* __restrict__ dL_dsh,
+    float* __restrict__ dL_dscale, float* __restrict__ dL_drot, int depth_grad) {
   constexpr int PB_STRIDE = NT + 1;  // floats per staging slot: NT (frame, Gaussian) values, + 1 so that slot k starts in bank k
-  __shared__ float s_stage[SL_COUNT * PB_STRIDE];
+  extern __shared__ __align__(16) float s_dyn[];  // [NG][M * 3] SH coefficients (with sh_smem), then the staging area
+  __shared__ __align__(8) uint64_t s_bar;
   pdl_wait();
   pdl_launch();
   const int FB = pb_frames_per_pass(F), NG = NT / FB;
   const int tid = threadIdx.x, wid = tid >> 5;
   const int fi = wid % FB, gl = (wid / FB) * 32 + (tid & 31);
-  const int g0 = blockIdx.x * NG, g = g0 + gl;
+  const int g0 = blockIdx.x * NG, g = g0 + gl, nval = min(NG, P - g0);
   // outputs summed over the frames (DGR_PF_* bits; with one frame every output is that frame's).  dL_dcolor
   // follows the colour input's bit, except with SH colours, where it is [P,3] scratch
   const int sum = F > 1 ? (DGR_PF_ALL & ~per_frame) : 0;
   const bool sum_col = dL_dcolor && F > 1 && (shs || (sum & DGR_PF_COLOR));
   const bool sum_sh = shs && (sum & DGR_PF_COLOR);
   const int ncoef = (D + 1) * (D + 1);
+  float* const s_stage = s_dyn + (sh_smem ? NG * 48 : 0);
   float* const stage = s_stage + fi * NG + gl;
+  if (sh_smem) {
+    if (tid == 0) {
+      mbar_init(&s_bar, 1);
+      mbar_fence_init();
+    }
+    __syncthreads();
+    if (tid == 0) {
+      mbar_expect_tx(&s_bar, nval * 192u);
+      tma_load_1d(s_dyn, shs + (size_t)g0 * 48, nval * 192u, &s_bar);
+    }
+  }
 
   for (int f0 = 0; f0 < F; f0 += FB) {
     const int f = f0 + fi;
@@ -467,33 +494,53 @@ __global__ void __launch_bounds__(NT, MIN_BLOCKS) preprocess_bwd_kernel(
       auto slab = [&](const float* p, int bit, int width) {
         return (per_frame & bit) ? p + (size_t)f * P * width : p;
       };
-      // staged when summed over the frames, else written to frame f's slab
-      auto put = [&](bool summed, float* out, int width, int slot, int c, float v) {
-        if (summed) stage[(slot + c) * PB_STRIDE] = v;
-        else out[fg * width + c] = v;
-      };
       const GeomWS gw = GeomWS::from(geom_ws + f * geom_stride, P);
+      // ---- every load of this (frame, Gaussian), issued before any of them is used
       const bool visible = (radii ? radii[fg] : gw.radii[g]) > 0;
-      // fetch + clear the accumulators written by render_bwd_kernel
       const float4 a0 = gw.grad_acc[3 * g + 0], a1 = gw.grad_acc[3 * g + 1], a2 = gw.grad_acc[3 * g + 2];
+      const float* mp = slab(means3D, DGR_PF_MEANS, 3) + 3 * g;
+      const float3 mean = make_float3(mp[0], mp[1], mp[2]);
+      float cov3D[6];
+      if (cov3D_precomp) {
+        const float* c = slab(cov3D_precomp, DGR_PF_COV, 6) + 6 * g;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) cov3D[k] = c[k];
+      } else {  // the workspace's rows are 8-byte aligned
+        const float2* c = reinterpret_cast<const float2*>(gw.cov3D + 6 * g);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          const float2 v = c[k];
+          cov3D[2 * k] = v.x;
+          cov3D[2 * k + 1] = v.y;
+        }
+      }
+      const float* sc_f = scales ? slab(scales, DGR_PF_SCALES, 3) : nullptr;
+      const float* rot_f = rotations ? slab(rotations, DGR_PF_ROTS, 4) : nullptr;
+      if (sc_f) {  // parked in the slots of their gradients until the EWA gradient is done (register budget)
+        const float4 q = __ldg(reinterpret_cast<const float4*>(rot_f) + g);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) stage[(SL_SCALE + k) * PB_STRIDE] = sc_f[3 * g + k];
+        stage[(SL_ROT + 0) * PB_STRIDE] = q.x;
+        stage[(SL_ROT + 1) * PB_STRIDE] = q.y;
+        stage[(SL_ROT + 2) * PB_STRIDE] = q.z;
+        stage[(SL_ROT + 3) * PB_STRIDE] = q.w;
+      }
+      // clear the accumulators written by render_bwd_kernel
       gw.grad_acc[3 * g + 0] = make_float4(0, 0, 0, 0);
       gw.grad_acc[3 * g + 1] = make_float4(0, 0, 0, 0);
       gw.grad_acc[3 * g + 2] = make_float4(0, 0, 0, 0);
-      const float2 dm2 = make_float2(a0.x, a0.y);
       const float3 dcon = make_float3(a0.z, a0.w, a1.x);  // (xx, xy, yy) slots .x .y .w of the reference float4
-      const float dop = a1.y;
-      const float3 dcol = make_float3(a1.z, a1.w, a2.x);
-
-      dL_dmean2D[3 * fg + 0] = dm2.x;
-      dL_dmean2D[3 * fg + 1] = dm2.y;
-      dL_dmean2D[3 * fg + 2] = 0.f;
+      // the 2D mean and colour gradients are read back from the staging area where they are used (fewer live
+      // registers through the EWA gradient)
+      stage[(SL_M2D + 0) * PB_STRIDE] = a0.x;
+      stage[(SL_M2D + 1) * PB_STRIDE] = a0.y;
+      stage[(SL_M2D + 2) * PB_STRIDE] = 0.f;
       if (dL_dconic) reinterpret_cast<float4*>(dL_dconic)[fg] = make_float4(dcon.x, dcon.y, 0.f, dcon.z);
-      put(sum & DGR_PF_OPAC, dL_dopacity, 1, SL_OPAC, 0, dop);
-      if (dL_dcolor) {
-        put(sum_col, dL_dcolor, 3, SL_COL, 0, dcol.x);
-        put(sum_col, dL_dcolor, 3, SL_COL, 1, dcol.y);
-        put(sum_col, dL_dcolor, 3, SL_COL, 2, dcol.z);
-      }
+      stage[SL_OPAC * PB_STRIDE] = a1.y;
+      stage[(SL_COL + 0) * PB_STRIDE] = a1.z;
+      stage[(SL_COL + 1) * PB_STRIDE] = a1.w;
+      stage[(SL_COL + 2) * PB_STRIDE] = a2.x;
+      stage[SL_MEAN * PB_STRIDE] = a2.y;  // dL/d(depth), until dL/dmean3D takes the slot
 
       float dcov[6] = {0, 0, 0, 0, 0, 0};
       float3 dmean = make_float3(0, 0, 0);
@@ -502,10 +549,7 @@ __global__ void __launch_bounds__(NT, MIN_BLOCKS) preprocess_bwd_kernel(
       float w[16], dRGB[3] = {0.f, 0.f, 0.f};
 #pragma unroll
       for (int k = 0; k < 16; ++k) w[k] = 0.f;
-      if (visible) {  // a culled Gaussian's gradients are zero
-        const float* mp = slab(means3D, DGR_PF_MEANS, 3) + 3 * g;
-        const float3 mean = make_float3(mp[0], mp[1], mp[2]);
-        const float* cov3D = cov3D_precomp ? slab(cov3D_precomp, DGR_PF_COV, 6) + 6 * g : gw.cov3D + 6 * g;
+      {
         const float* view = views + 16 * f;
         const float* proj = projs + 16 * f;
         const float focal_x = cams.fx[f], focal_y = cams.fy[f], tan_fovx = cams.tanx[f], tan_fovy = cams.tany[f];
@@ -568,6 +612,7 @@ __global__ void __launch_bounds__(NT, MIN_BLOCKS) preprocess_bwd_kernel(
         const float mul1 = (proj[0] * mean.x + proj[4] * mean.y + proj[8] * mean.z + proj[12]) * m_w * m_w;
         const float mul2 = (proj[1] * mean.x + proj[5] * mean.y + proj[9] * mean.z + proj[13]) * m_w * m_w;
         float3 dm;
+        const float2 dm2 = make_float2(stage[SL_M2D * PB_STRIDE], stage[(SL_M2D + 1) * PB_STRIDE]);
         dm.x = (proj[0] * m_w - proj[3] * mul1) * dm2.x + (proj[1] * m_w - proj[3] * mul2) * dm2.y;
         dm.y = (proj[4] * m_w - proj[7] * mul1) * dm2.x + (proj[5] * m_w - proj[7] * mul2) * dm2.y;
         dm.z = (proj[8] * m_w - proj[11] * mul1) * dm2.x + (proj[9] * m_w - proj[11] * mul2) * dm2.y;
@@ -577,27 +622,18 @@ __global__ void __launch_bounds__(NT, MIN_BLOCKS) preprocess_bwd_kernel(
         // depth map: dL/d(depth) (grad_acc float 9) through depth = p_view.z, the third row of the view
         // transform (xform4x3).  Only when the backward carries one: adding 0 would turn -0 into +0
         if (depth_grad) {
-          dmean.x += a2.y * view[2];
-          dmean.y += a2.y * view[6];
-          dmean.z += a2.y * view[10];
+          const float dd = stage[SL_MEAN * PB_STRIDE];
+          dmean.x += dd * view[2];
+          dmean.y += dd * view[6];
+          dmean.z += dd * view[10];
         }
 
-        // ---------------- SH colour (backward.cu:20-139, 383-385)
-        if (shs) {
-          const float3 cp = make_float3(cam_poses[3 * f], cam_poses[3 * f + 1], cam_poses[3 * f + 2]);
-          float sh[48];
-          load_sh(slab(shs, DGR_PF_COLOR, M * 3), g, M, ncoef, sh);
-          const float3 dms = sh_backward(D, mean, cp, sh, gw.clamped + 3 * g, dcol, w, dRGB);
-          dmean.x += dms.x;
-          dmean.y += dms.y;
-          dmean.z += dms.z;
-        }
-        const float* sc_f = scales ? slab(scales, DGR_PF_SCALES, 3) : nullptr;
-        const float* rot_f = rotations ? slab(rotations, DGR_PF_ROTS, 4) : nullptr;
         // ---------------- 3D covariance -> scale / rotation (backward.cu:279-341)
         if (sc_f) {
-          const float3 sc = make_float3(sc_f[3 * g], sc_f[3 * g + 1], sc_f[3 * g + 2]);
-          const float4 q = __ldg(reinterpret_cast<const float4*>(rot_f) + g);
+          const float3 sc = make_float3(stage[SL_SCALE * PB_STRIDE], stage[(SL_SCALE + 1) * PB_STRIDE],
+                                        stage[(SL_SCALE + 2) * PB_STRIDE]);
+          const float4 q = make_float4(stage[SL_ROT * PB_STRIDE], stage[(SL_ROT + 1) * PB_STRIDE],
+                                       stage[(SL_ROT + 2) * PB_STRIDE], stage[(SL_ROT + 3) * PB_STRIDE]);
           const float r = q.x, x = q.y, y = q.z, z = q.w;
           Mat3 R;
           quat_to_R(q, R);
@@ -647,80 +683,121 @@ __global__ void __launch_bounds__(NT, MIN_BLOCKS) preprocess_bwd_kernel(
           drot.w = 2 * r * (dMt.c[0][1] - dMt.c[1][0]) + 2 * x * (dMt.c[2][0] + dMt.c[0][2]) +
                    2 * y * (dMt.c[1][2] + dMt.c[2][1]) - 4 * z * (dMt.c[1][1] + dMt.c[0][0]);
         }
-      }
-      if (sum_sh) {
+        // a culled Gaussian's gradients are zero: the visibility test selects the results
+        auto vis = [&](float v) { return visible ? v : 0.f; };
 #pragma unroll
-        for (int k = 0; k < 16; ++k) put(true, nullptr, 0, SL_W, k, w[k]);
+        for (int k = 0; k < 6; ++k) stage[(SL_COV + k) * PB_STRIDE] = vis(dcov[k]);
+        stage[(SL_SCALE + 0) * PB_STRIDE] = vis(dscale.x);
+        stage[(SL_SCALE + 1) * PB_STRIDE] = vis(dscale.y);
+        stage[(SL_SCALE + 2) * PB_STRIDE] = vis(dscale.z);
+        stage[(SL_ROT + 0) * PB_STRIDE] = vis(drot.x);
+        stage[(SL_ROT + 1) * PB_STRIDE] = vis(drot.y);
+        stage[(SL_ROT + 2) * PB_STRIDE] = vis(drot.z);
+        stage[(SL_ROT + 3) * PB_STRIDE] = vis(drot.w);
+
+        // ---------------- SH colour (backward.cu:20-139, 383-385)
+        if (shs) {
+          const float3 cp = make_float3(cam_poses[3 * f], cam_poses[3 * f + 1], cam_poses[3 * f + 2]);
+          float sh[48];
+          if (!sh_smem) {
+            load_sh(slab(shs, DGR_PF_COLOR, M * 3), g, M, ncoef, sh);
+          } else {
+            mbar_wait(&s_bar, 0);
+            const float4* v = reinterpret_cast<const float4*>(s_dyn + gl * 48);
 #pragma unroll
-        for (int ch = 0; ch < 3; ++ch) put(true, nullptr, 0, SL_RGB, ch, dRGB[ch]);
-      } else if (shs) {
-        float* dst = dL_dsh + fg * M * 3;
-        if (M == 16) {
-#pragma unroll
-          for (int i = 0; i < 12; ++i) {
-            float o[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) o[j] = (4 * i + j) / 3 < ncoef ? w[(4 * i + j) / 3] * dRGB[(4 * i + j) % 3] : 0.f;
-            reinterpret_cast<float4*>(dst)[i] = make_float4(o[0], o[1], o[2], o[3]);
+            for (int i = 0; i < 12; ++i) {
+              const float4 t = v[i];
+              sh[4 * i + 0] = t.x;
+              sh[4 * i + 1] = t.y;
+              sh[4 * i + 2] = t.z;
+              sh[4 * i + 3] = t.w;
+            }
           }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 48; ++i)
-            if (i < M * 3) dst[i] = i / 3 < ncoef ? w[i / 3] * dRGB[i % 3] : 0.f;
+          const float3 dcol = make_float3(stage[SL_COL * PB_STRIDE], stage[(SL_COL + 1) * PB_STRIDE],
+                                          stage[(SL_COL + 2) * PB_STRIDE]);
+          const float3 dms = sh_backward(D, mean, cp, sh, gw.clamped + 3 * g, dcol, w, dRGB);
+          dmean.x += dms.x;
+          dmean.y += dms.y;
+          dmean.z += dms.z;
         }
-      }
-      put(sum & DGR_PF_MEANS, dL_dmean3D, 3, SL_MEAN, 0, dmean.x);
-      put(sum & DGR_PF_MEANS, dL_dmean3D, 3, SL_MEAN, 1, dmean.y);
-      put(sum & DGR_PF_MEANS, dL_dmean3D, 3, SL_MEAN, 2, dmean.z);
-      if (dL_dcov3D) {
 #pragma unroll
-        for (int k = 0; k < 6; ++k) put(sum & DGR_PF_COV, dL_dcov3D, 6, SL_COV, k, dcov[k]);
+        for (int k = 0; k < 16; ++k) stage[(SL_W + k) * PB_STRIDE] = vis(w[k]);
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) stage[(SL_RGB + ch) * PB_STRIDE] = vis(dRGB[ch]);
+        stage[(SL_MEAN + 0) * PB_STRIDE] = vis(dmean.x);
+        stage[(SL_MEAN + 1) * PB_STRIDE] = vis(dmean.y);
+        stage[(SL_MEAN + 2) * PB_STRIDE] = vis(dmean.z);
       }
-      put(sum & DGR_PF_SCALES, dL_dscale, 3, SL_SCALE, 0, dscale.x);
-      put(sum & DGR_PF_SCALES, dL_dscale, 3, SL_SCALE, 1, dscale.y);
-      put(sum & DGR_PF_SCALES, dL_dscale, 3, SL_SCALE, 2, dscale.z);
-      put(sum & DGR_PF_ROTS, dL_drot, 4, SL_ROT, 0, drot.x);
-      put(sum & DGR_PF_ROTS, dL_drot, 4, SL_ROT, 1, drot.y);
-      put(sum & DGR_PF_ROTS, dL_drot, 4, SL_ROT, 2, drot.z);
-      put(sum & DGR_PF_ROTS, dL_drot, 4, SL_ROT, 3, drot.w);
+    }
+    // ---- per-frame outputs: each warp writes the rows of its own 32 Gaussians as soon as it has staged them
+    // (element e = q * width + c of the warp's slice is row q, column c: every store of the warp covers 128
+    // consecutive bytes), without waiting for the rest of the block
+    if (f < F) {  // uniform per warp
+      __syncwarp();
+      const int gw0 = (wid / FB) * 32, nw = min(32, P - g0 - gw0);
+      const float* ws = s_stage + fi * NG + gw0;
+      auto own = [&](float* out, int width, auto value) {
+        float* dst = out + ((size_t)f * P + g0 + gw0) * width;
+#pragma unroll 4
+        for (int j = 0; j < width; ++j) {
+          const int e = (tid & 31) + 32 * j, q = e / width, c = e - q * width;
+          if (q < nw) dst[e] = value(ws, q, c);
+        }
+      };
+      auto staged = [](int slot) {
+        return [=](const float* st, int q, int c) { return st[(slot + c) * PB_STRIDE + q]; };
+      };
+      own(dL_dmean2D, 3, staged(SL_M2D));
+      if (!(sum & DGR_PF_OPAC)) own(dL_dopacity, 1, staged(SL_OPAC));
+      if (dL_dcolor && !sum_col) own(dL_dcolor, 3, staged(SL_COL));
+      if (!(sum & DGR_PF_MEANS)) own(dL_dmean3D, 3, staged(SL_MEAN));
+      if (dL_dcov3D && !(sum & DGR_PF_COV)) own(dL_dcov3D, 6, staged(SL_COV));
+      if (!(sum & DGR_PF_SCALES)) own(dL_dscale, 3, staged(SL_SCALE));
+      if (!(sum & DGR_PF_ROTS)) own(dL_drot, 4, staged(SL_ROT));
+      // dL_dsh[k][ch] = w[k] dRGB[ch]; 0 for the coefficients k >= ncoef that the SH degree does not use
+      if (shs && !sum_sh)
+        own(dL_dsh, 3 * M, [=](const float* st, int q, int c) {
+          const int k = c / 3;
+          return k < ncoef ? __fmul_rn(st[(SL_W + k) * PB_STRIDE + q], st[(SL_RGB + c - 3 * k) * PB_STRIDE + q]) : 0.f;
+        });
+      __syncwarp();
     }
     if (!sum && !sum_col) continue;  // uniform: nothing is summed over the frames
     __syncthreads();
-    // ---- sum this pass's frames into the block's rows of each summed output: row q, column c is
-    // element e = q * width + c of the block's slice (the warp stores 128 consecutive bytes); a pass after
-    // the first continues from the value the previous pass stored
-    const int nf = min(FB, F - f0), nval = min(NG, P - g0);
-    auto sum_frames = [&](float* out, int width, int slot) {
+    // ---- outputs summed over the frames: the block sums this pass's frames into its rows, in frame order,
+    // continuing from the value the previous pass stored.  value(q, c, i) is frame i's staged value
+    const int nf = min(FB, F - f0);
+    auto sum_rows = [&](float* out, int width, auto value) {
       float* dst = out + (size_t)g0 * width;
       for (int e = tid; e < nval * width; e += NT) {
-        const int q = e / width;
-        const float* s = s_stage + (slot + e - q * width) * PB_STRIDE + q;
-        float acc = f0 ? dst[e] : s[0];
-        for (int i = f0 ? 0 : 1; i < nf; ++i) acc = acc + s[i * NG];
+        const int q = e / width, c = e - q * width;
+        float v[8];  // FB <= 8: every frame's value is read before the sequential sum
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = i < nf ? value(q, c, i) : 0.f;
+        float acc = f0 ? dst[e] : v[0];
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+          if (i < nf && (f0 || i > 0)) acc = acc + v[i];
         dst[e] = acc;
       }
     };
-    if (sum & DGR_PF_OPAC) sum_frames(dL_dopacity, 1, SL_OPAC);
-    if (sum_col) sum_frames(dL_dcolor, 3, SL_COL);
-    if (sum & DGR_PF_MEANS) sum_frames(dL_dmean3D, 3, SL_MEAN);
-    if ((sum & DGR_PF_COV) && dL_dcov3D) sum_frames(dL_dcov3D, 6, SL_COV);
-    if (sum & DGR_PF_SCALES) sum_frames(dL_dscale, 3, SL_SCALE);
-    if (sum & DGR_PF_ROTS) sum_frames(dL_drot, 4, SL_ROT);
-    if (sum_sh) {  // dL_dsh[k][ch] = sum over frames of w[k] dRGB[ch], each product rounded before it is added
-      const int width = 3 * M;
-      float* dst = dL_dsh + (size_t)g0 * width;
-      for (int e = tid; e < nval * width; e += NT) {
-        const int q = e / width, c = e - q * width, k = c / 3;
-        const float* sw = s_stage + (SL_W + k) * PB_STRIDE + q;
-        const float* sd = s_stage + (SL_RGB + c - 3 * k) * PB_STRIDE + q;
-        float acc = 0.f;
-        if (k < ncoef) {
-          acc = f0 ? dst[e] : __fmul_rn(sw[0], sd[0]);
-          for (int i = f0 ? 0 : 1; i < nf; ++i) acc = __fadd_rn(acc, __fmul_rn(sw[i * NG], sd[i * NG]));
-        }
-        dst[e] = acc;
-      }
-    }
+    auto summed = [&](int slot) {
+      return [=](int q, int c, int i) { return s_stage[(slot + c) * PB_STRIDE + i * NG + q]; };
+    };
+    if (sum & DGR_PF_OPAC) sum_rows(dL_dopacity, 1, summed(SL_OPAC));
+    if (sum_col) sum_rows(dL_dcolor, 3, summed(SL_COL));
+    if (sum & DGR_PF_MEANS) sum_rows(dL_dmean3D, 3, summed(SL_MEAN));
+    if ((sum & DGR_PF_COV) && dL_dcov3D) sum_rows(dL_dcov3D, 6, summed(SL_COV));
+    if (sum & DGR_PF_SCALES) sum_rows(dL_dscale, 3, summed(SL_SCALE));
+    if (sum & DGR_PF_ROTS) sum_rows(dL_drot, 4, summed(SL_ROT));
+    // each product rounded before it is added; 0 for k >= ncoef
+    if (sum_sh)
+      sum_rows(dL_dsh, 3 * M, [=](int q, int c, int i) {
+        const int k = c / 3;
+        return k < ncoef ? __fmul_rn(s_stage[(SL_W + k) * PB_STRIDE + i * NG + q],
+                                     s_stage[(SL_RGB + c - 3 * k) * PB_STRIDE + i * NG + q])
+                         : 0.f;
+      });
     __syncthreads();  // the next pass overwrites the staging area
   }
 }
@@ -768,10 +845,19 @@ cudaError_t launch_preprocess_bwd(const BwdArgs& a, cudaStream_t s) {
     c.fx[f] = a.W / (2.0f * a.tan_fovx[f]);
     c.fy[f] = a.H / (2.0f * a.tan_fovy[f]);
   }
+  auto one = preprocess_bwd_kernel<128, 3>, batch = preprocess_bwd_kernel<256, 2>;
+  static unsigned long long attr = 0;  // per device
+  if (once_per_device(attr)) {
+    // the largest staging area + SH tile (2 or 3 frames: 128 Gaussians per block) exceeds 48 KB
+    cudaFuncSetAttribute(one, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pb_smem_bytes(128, 1, 16, true));
+    cudaFuncSetAttribute(batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pb_smem_bytes(256, 2, 16, true));
+  }
+  // 16 SH coefficients per Gaussian are read as 16-byte vectors throughout (load_sh): 192-byte rows, aligned
+  const bool sh_smem = a.shs && a.M == 16 && (a.F == 1 || !(a.per_frame & DGR_PF_COLOR));
   const int nt = a.F == 1 ? 128 : 256, ng = nt / pb_frames_per_pass(a.F);
   g_prof.begin(6, s);
-  launch_pdl(a.F == 1 ? preprocess_bwd_kernel<128, 3> : preprocess_bwd_kernel<256, 2>, dim3((a.P + ng - 1) / ng),
-             dim3(nt), 0, s, a.F, a.P, a.D, a.M, a.per_frame, a.means3D, a.radii, a.shs, a.scales, a.rotations,
+  launch_pdl(a.F == 1 ? one : batch, dim3((a.P + ng - 1) / ng), dim3(nt), pb_smem_bytes(nt, a.F, a.M, sh_smem), s,
+             a.F, a.P, a.D, a.M, a.per_frame, a.means3D, a.radii, a.shs, sh_smem ? 1 : 0, a.scales, a.rotations,
              a.scale_modifier, a.cov3D_precomp, a.viewmatrix, a.projmatrix, a.cam_pos, c, (char*)a.geom_ws,
              a.geom_stride, a.dL_dmean2D, a.dL_dconic, a.dL_dopacity, a.dL_dcolor, a.dL_dmean3D, a.dL_dcov3D,
              a.dL_dsh, a.dL_dscale, a.dL_drot, a.dL_ddepth ? 1 : 0);
