@@ -16,7 +16,11 @@ reference config): branch_w / branch_v run as one 6-row head of the same kernel 
 (utils/rigid_utils.py) is elementwise torch on the [N,6] result.
 
 The packed bf16 operands are cached per module and rebuilt only when a parameter changed (tensor
-version counters), i.e. once per optimiser step, not once per forward.
+version counters), i.e. once per optimiser step, not once per forward.  Optimiser steps, in-place edits under
+torch.no_grad(), load_state_dict and assigning a new Parameter are all seen (tests/test_mlp_tiles.py).  A write
+through `.data` (`p.data.mul_(2)`) is NOT: it leaves the version counter unchanged, and a module that has run a
+forward keeps using the weights it packed before the write.  Update weights in place under torch.no_grad()
+instead.  (The `.data` writes in DeformNetworkNormalSep's constructor run before any forward.)
 """
 import ctypes
 import os
