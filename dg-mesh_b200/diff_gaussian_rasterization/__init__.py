@@ -205,13 +205,48 @@ def _surface_ws_bytes(W, H):
     return n.value
 
 
+_null_segments = {}
+
+
+def _enqueue(base, parts):
+    """Call the narrowest entry point `base` + suffix that takes every argument segment in use.
+
+    parts: (suffix, args) in ABI order; suffix None for the arguments every variant takes, otherwise an optional
+    segment, args None when it is not in use.  The variants nest in that order: each one's argument list is the next
+    narrower one's with its segment inserted (_dgm_lib.SIGNATURES), so every segment up to the widest one in use is
+    passed, an unused one as the zeros / NULLs of its types there."""
+    name = base
+    for suffix, args in parts:
+        if suffix is not None and args is not None:
+            name = base + suffix
+    out, narrower, done = [], base, name == base
+    for suffix, args in parts:
+        if suffix is None:
+            out.extend(args)
+        elif not done:
+            wider = base + suffix
+            out.extend(args if args is not None else _null_segment(wider, narrower, len(out)))
+            narrower, done = wider, wider == name
+    _dgm_lib.check(getattr(_dgm_lib.lib(), name)(*out), name)
+
+
+def _null_segment(name, narrower, at):
+    """The zeros / NULLs of the segment that `name` inserts into `narrower`'s arguments at position `at`."""
+    v = _null_segments.get(name)
+    if v is None:
+        sig = _dgm_lib.SIGNATURES
+        n = len(sig[name][1]) - len(sig[narrower][1])
+        v = _null_segments[name] = tuple(None if t is _dgm_lib.P else 0.0 if t is _dgm_lib.c_float else 0
+                                         for t in sig[name][1][at:at + n])
+    return v
+
+
 def _raw_forward(bg, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                  projmatrix, tan_fovx, tan_fovy, H, W, sh, degree, campos, prefiltered, R_cap, notify=None,
                  lo=0.0, hi=0.0, out=None, max_tile=0, maps=None, nrm=None, surf=None):
-    """One enqueue of dgr_forward (dgr_forward_aux when `maps` = (depth, alpha) [1,H,W] tensors to write;
-    dgr_forward_nrm when also `nrm` = (normals [P,3], normal map [3,H,W]); dgr_forward_surf when also `surf` =
-    (near, far, median [1,H,W], distortion [1,H,W])).  Returns (color, radii, workspace)."""
-    lib = _dgm_lib.lib()
+    """One enqueue of the dgr_forward entry point (see `_enqueue`) that also writes `maps` = (depth, alpha) [1,H,W]
+    and, with the maps, `nrm` = (normals [P,3], normal map [3,H,W]) and `surf` = (near, far, median [1,H,W],
+    distortion [1,H,W]).  Returns (color, radii, workspace)."""
     if means3D.ndim != 2 or means3D.shape[1] != 3:
         raise ValueError("means3D must have dimensions (num_points, 3)")  # rasterize_points.cu:57-59
     dev = means3D.device
@@ -230,26 +265,17 @@ def _raw_forward(bg, means3D, colors, opacity, scales, rotations, scale_modifier
     tail = (ws.geom, ws.gb, ws.binning, ws.bb, R_cap, ws.img, ws.ib, ws.status,
             notify.host_ptr if notify else None, notify.event if notify else None, lo, hi, int(max_tile),
             _dgm_lib.stream_ptr())
-    if surf is not None:
-        nb = _normal_ws_bytes(P, R_cap) if nrm is not None else 0
-        if nrm is not None:
-            ws.nrm = torch.empty((nb,), dtype=torch.uint8, device=dev)
-        sb = _surface_ws_bytes(W, H)
-        ws.surf = torch.empty((sb,), dtype=torch.uint8, device=dev)
-        n_in, n_map = nrm if nrm is not None else (None, None)
-        _dgm_lib.check(lib.dgr_forward_surf(*head, p(maps[0]), p(maps[1]), p(n_in), p(n_map),
-                                            ws.nrm.data_ptr() if nrm is not None else None, nb, float(surf[0]),
-                                            float(surf[1]), p(surf[2]), p(surf[3]), ws.surf.data_ptr(), sb, *tail),
-                       "dgr_forward_surf")
-    elif nrm is not None:
+    nrm_args = surf_args = None
+    if nrm is not None:
         nb = _normal_ws_bytes(P, R_cap)
         ws.nrm = torch.empty((nb,), dtype=torch.uint8, device=dev)
-        _dgm_lib.check(lib.dgr_forward_nrm(*head, p(maps[0]), p(maps[1]), p(nrm[0]), p(nrm[1]), ws.nrm.data_ptr(), nb,
-                                           *tail), "dgr_forward_nrm")
-    elif maps is None:
-        _dgm_lib.check(lib.dgr_forward(*head, *tail), "dgr_forward")
-    else:
-        _dgm_lib.check(lib.dgr_forward_aux(*head, p(maps[0]), p(maps[1]), *tail), "dgr_forward_aux")
+        nrm_args = (p(nrm[0]), p(nrm[1]), ws.nrm.data_ptr(), nb)
+    if surf is not None:
+        sb = _surface_ws_bytes(W, H)
+        ws.surf = torch.empty((sb,), dtype=torch.uint8, device=dev)
+        surf_args = (float(surf[0]), float(surf[1]), p(surf[2]), p(surf[3]), ws.surf.data_ptr(), sb)
+    _enqueue("dgr_forward", ((None, head), ("_aux", None if maps is None else (p(maps[0]), p(maps[1]))),
+                             ("_nrm", nrm_args), ("_surf", surf_args), (None, tail)))
     return color, radii, ws
 
 
@@ -264,20 +290,23 @@ class _RasterizeGaussians(torch.autograd.Function):
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 raster_settings):
         return _RasterizeGaussians._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                        cov3Ds_precomp, raster_settings, None)
+                                        cov3Ds_precomp, raster_settings)
 
     @staticmethod
     def backward(ctx, grad_out_color, _):
-        return _RasterizeGaussians._bwd(ctx, grad_out_color, None, None)
+        return _RasterizeGaussians._bwd(ctx, grad_out_color)   # its last entry, dL/dnormals, is None here
 
     @staticmethod
     def _fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-             raster_settings, maps, nrm=None, surf=None, saved=()):
+             raster_settings, maps=None, nrm=None, surf=None, cams=None, saved=()):
         """maps: None (colour only) or the (depth, alpha) [1,H,W] tensors the forward writes as well.
         nrm: None, or (normals [P,3], normal map [3,H,W]) for the normal map (with maps).
         surf: None, or (near, far, median [1,H,W], distortion [1,H,W]) for the surface maps (with maps).
+        cams: None (the settings' camera), or the (viewmatrix, projmatrix, campos) to use instead.
         saved: more tensors to save for the backward, after (means3D, radii)."""
         rs = raster_settings
+        if cams is not None:
+            rs = rs._replace(viewmatrix=cams[0].detach(), projmatrix=cams[1].detach(), campos=cams[2].detach())
         means3D = _f32c(means3D, "means3D")
         if means3D is None:
             raise ValueError("means3D must have dimensions (num_points, 3)")
@@ -312,19 +341,18 @@ class _RasterizeGaussians(torch.autograd.Function):
         return color, radii
 
     @staticmethod
-    def _bwd(ctx, grad_out_color, grad_depth, grad_alpha, cam=None, nrm=None, surf=None, abs_out=None):
+    def _bwd(ctx, grad_out_color, grad_depth=None, grad_alpha=None, cam=None, nrm=None, surf=None, abs_out=None):
         """grad_depth / grad_alpha: None, or the upstream gradients of the maps (None = unused by the loss).
         cam: None, or the _CameraGrads the backward writes the camera gradients to.
-        nrm: None, or (upstream gradient of the normal map, whether dL/dnormals is needed); then the result has a
-        tenth entry, dL/dnormals [P,3] (or None).
+        nrm: None, or (upstream gradient of the normal map, whether dL/dnormals is needed).
         surf: None, or (near, far, upstream gradients of the median-depth and distortion maps, each None when
         unused, not both).
-        abs_out: None, or the [P,3] tensor the backward writes the absolute screen-space gradient to."""
+        abs_out: None, or the [P,3] tensor the backward writes the absolute screen-space gradient to.
+        Returns the eight Gaussian inputs' gradients in the reference's order, then dL/dnormals [P,3] (or None)."""
         rs = ctx.raster_settings
         bg, sh, col, opac, sc, rot, cov, view, proj, campos = ctx.tensors
         means3D, radii = ctx.saved_tensors[:2]
         ws = ctx.ws
-        lib = _dgm_lib.lib()
         P = means3D.shape[0]
         H, W = int(rs.image_height), int(rs.image_width)
         M = int(sh.shape[1]) if sh is not None else 0
@@ -352,77 +380,26 @@ class _RasterizeGaussians(torch.autograd.Function):
         head = (P, rs.sh_degree, M, p(bg), W, H, p(means3D), p(sh), p(col), p(sc), float(rs.scale_modifier), p(rot),
                 p(cov), p(view), p(proj), p(campos), float(rs.tanfovx), float(rs.tanfovy), p(radii), ws.geom,
                 ws.binning, ws.R_cap, ws.img, p(dpix))
-        tail = (ptrs[0], None, ptrs[2], ptrs[3], ptrs[4], ptrs[5], ptrs[8] if M else None, ptrs[6], ptrs[7],
-                _dgm_lib.stream_ptr())
-        dnormals = None
-        if surf is not None or abs_out is not None:
-            gd, ga = _f32c(grad_depth, "grad_depth"), _f32c(grad_alpha, "grad_alpha")
-            gn = _f32c(nrm[0], "grad_normal") if nrm is not None else None
-            if nrm is not None and nrm[1]:
-                dnormals = torch.empty((P, 3), dtype=torch.float32, device=means3D.device)
-            cargs = cam.args() if cam is not None else (None, None, None, None, 0)
-            sargs = (0.0, 0.0, None, None, None)
-            if surf is not None:
-                sargs = (float(surf[0]), float(surf[1]), p(_f32c(surf[2], "grad_median_depth")),
-                         p(_f32c(surf[3], "grad_distortion")), ws.surf.data_ptr())
-            _dgm_lib.check(lib.dgr_backward_abs(*head, p(gd), p(ga), *tail[:-1], *cargs, p(gn), p(dnormals),
-                                                ws.nrm.data_ptr() if gn is not None else None, *sargs, p(abs_out),
-                                                tail[-1]), "dgr_backward_abs")
-        elif nrm is not None:
-            gd, ga, gn = _f32c(grad_depth, "grad_depth"), _f32c(grad_alpha, "grad_alpha"), _f32c(nrm[0], "grad_normal")
+        grads = (ptrs[0], None, ptrs[2], ptrs[3], ptrs[4], ptrs[5], ptrs[8] if M else None, ptrs[6], ptrs[7])
+        aux = nrm_args = surf_args = dnormals = None
+        if grad_depth is not None or grad_alpha is not None:
+            aux = (p(_f32c(grad_depth, "grad_depth")), p(_f32c(grad_alpha, "grad_alpha")))
+        if nrm is not None:
             if nrm[1]:
                 dnormals = torch.empty((P, 3), dtype=torch.float32, device=means3D.device)
-            cargs = cam.args() if cam is not None else (None, None, None, None, 0)
-            _dgm_lib.check(lib.dgr_backward_nrm(*head, p(gd), p(ga), *tail[:-1], *cargs, p(gn), p(dnormals),
-                                                ws.nrm.data_ptr(), tail[-1]), "dgr_backward_nrm")
-        elif cam is not None:
-            gd, ga = _f32c(grad_depth, "grad_depth"), _f32c(grad_alpha, "grad_alpha")
-            _dgm_lib.check(lib.dgr_backward_cam(*head, p(gd), p(ga), *tail[:-1], *cam.args(), tail[-1]),
-                           "dgr_backward_cam")
-        elif grad_depth is None and grad_alpha is None:
-            _dgm_lib.check(lib.dgr_backward(*head, *tail), "dgr_backward")
-        else:
-            gd, ga = _f32c(grad_depth, "grad_depth"), _f32c(grad_alpha, "grad_alpha")
-            _dgm_lib.check(lib.dgr_backward_aux(*head, p(gd), p(ga), *tail), "dgr_backward_aux")
+            nrm_args = (p(_f32c(nrm[0], "grad_normal")), p(dnormals), ws.nrm.data_ptr())
+        if surf is not None:
+            surf_args = (float(surf[0]), float(surf[1]), p(_f32c(surf[2], "grad_median_depth")),
+                         p(_f32c(surf[3], "grad_distortion")), ws.surf.data_ptr())
+        _enqueue("dgr_backward", ((None, head), ("_aux", aux), (None, grads),
+                                  ("_cam", None if cam is None else cam.args()), ("_nrm", nrm_args),
+                                  ("_surf", surf_args), ("_abs", None if abs_out is None else (p(abs_out),)),
+                                  (None, (_dgm_lib.stream_ptr(),))))
         # same ordering as the reference (:143-153)
-        g = (gview(4, P, 3), gview(0, P, 3) if ctx.has_m2d else None,
-             gview(8, P, M, 3) if sh is not None else None, gview(3, P, 3) if col is not None else None,
-             gview(2, P, 1), gview(6, P, 3) if sc is not None else None,
-             gview(7, P, 4) if rot is not None else None, gview(5, P, 6) if cov is not None else None, None)
-        return g if nrm is None else g + (dnormals,)
-
-
-class _RasterizeGaussiansDepthAlpha(torch.autograd.Function):
-    """`_RasterizeGaussians` that also returns the depth map sum_i d_i alpha_i T_i and the alpha map
-    1 - T_final, [1,H,W] each.  Gradients are not materialised: a map the loss does not use arrives as None
-    and is handed to the library as NULL, so a colour-only loss runs the colour-only backward."""
-
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings):
-        ctx.set_materialize_grads(False)
-        H, W = int(raster_settings.image_height), int(raster_settings.image_width)
-        maps = tuple(torch.empty((1, H, W), dtype=torch.float32, device=means3D.device) for _ in range(2))
-        color, radii = _RasterizeGaussians._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales,
-                                                rotations, cov3Ds_precomp, raster_settings, maps)
-        return color, radii, maps[0], maps[1]
-
-    @staticmethod
-    def backward(ctx, grad_out_color, _, grad_depth, grad_alpha):
-        return _RasterizeGaussians._bwd(ctx, grad_out_color, grad_depth, grad_alpha)
-
-
-def _abs_input(ctx, means2D_abs, shape):
-    """Check the optional means2D_abs input (the last forward input) of a Function: it has `shape`, the shape of the
-    absolute screen-space gradient its .grad receives ([P,3], or [F,P,3] for a batch)."""
-    if means2D_abs is not None and tuple(means2D_abs.shape) != tuple(shape):
-        raise ValueError(f"means2D_abs must have dimensions {tuple(shape)}")
-    ctx.abs_shape = tuple(shape)
-
-
-def _abs_output(ctx, dev):
-    """The tensor the backward writes the absolute screen-space gradient to when means2D_abs needs a gradient."""
-    return torch.empty(ctx.abs_shape, dtype=torch.float32, device=dev) if ctx.needs_input_grad[-1] else None
+        return (gview(4, P, 3), gview(0, P, 3) if ctx.has_m2d else None,
+                gview(8, P, M, 3) if sh is not None else None, gview(3, P, 3) if col is not None else None,
+                gview(2, P, 1), gview(6, P, 3) if sc is not None else None,
+                gview(7, P, 4) if rot is not None else None, gview(5, P, 6) if cov is not None else None, dnormals)
 
 
 class _CameraGrads:
@@ -448,126 +425,6 @@ class _CameraGrads:
         """The gradients in the shapes of the camera tensors (None where none is needed)."""
         return tuple(g.reshape(shape) if need else None
                      for g, shape, need in zip((self.view, self.proj, self.campos), shapes, self.need))
-
-
-class _RasterizeGaussiansCam(torch.autograd.Function):
-    """`_RasterizeGaussians` (depth_alpha: `_RasterizeGaussiansDepthAlpha`) with the camera as explicit inputs:
-    viewmatrix [4,4], projmatrix [4,4] and campos [3] replace the settings' tensors and receive gradients.
-    Gradients are not materialised; when no camera tensor needs a gradient the backward is the existing one."""
-
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, viewmatrix,
-                projmatrix, campos, raster_settings, depth_alpha, means2D_abs=None):
-        ctx.set_materialize_grads(False)
-        _abs_input(ctx, means2D_abs, (means3D.shape[0], 3))
-        rs = raster_settings._replace(viewmatrix=viewmatrix.detach(), projmatrix=projmatrix.detach(),
-                                      campos=campos.detach())
-        maps = None
-        if depth_alpha:
-            H, W = int(rs.image_height), int(rs.image_width)
-            maps = tuple(torch.empty((1, H, W), dtype=torch.float32, device=means3D.device) for _ in range(2))
-        color, radii = _RasterizeGaussians._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales,
-                                                rotations, cov3Ds_precomp, rs, maps)
-        ctx.cam_shapes = (viewmatrix.shape, projmatrix.shape, campos.shape)
-        return (color, radii) + (maps if depth_alpha else ())
-
-    @staticmethod
-    def backward(ctx, grad_out_color, _, grad_depth=None, grad_alpha=None):
-        need = tuple(ctx.needs_input_grad[8:11])
-        cam = _CameraGrads(1, ctx.saved_tensors[0].shape[0], ctx.saved_tensors[0].device, need) if any(need) else None
-        ab = _abs_output(ctx, ctx.saved_tensors[0].device)
-        g = _RasterizeGaussians._bwd(ctx, grad_out_color, grad_depth, grad_alpha, cam, abs_out=ab)
-        return g[:8] + (cam.grads(ctx.cam_shapes) if cam else (None, None, None)) + (None, None, ab)
-
-
-class _RasterizeGaussiansNormal(torch.autograd.Function):
-    """`_RasterizeGaussiansDepthAlpha` + the normal map sum_i n_i alpha_i T_i [3,H,W] of `normals` [P,3], with the
-    camera as explicit inputs (see _RasterizeGaussiansCam; pass detached tensors for no camera gradient).
-    Gradients are not materialised: a loss that does not use the normal map runs the depth / alpha (or colour-only)
-    backward, and the normal map's gradient reaches the library as NULL."""
-
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, normals,
-                viewmatrix, projmatrix, campos, raster_settings, means2D_abs=None):
-        ctx.set_materialize_grads(False)
-        _abs_input(ctx, means2D_abs, (means3D.shape[0], 3))
-        rs = raster_settings._replace(viewmatrix=viewmatrix.detach(), projmatrix=projmatrix.detach(),
-                                      campos=campos.detach())
-        H, W = int(rs.image_height), int(rs.image_width)
-        nrm_in = _f32c(normals, "normals")
-        if nrm_in is None or nrm_in.shape != (means3D.shape[0], 3):
-            raise ValueError("normals must have dimensions (num_points, 3)")
-        maps = tuple(torch.empty((1, H, W), dtype=torch.float32, device=means3D.device) for _ in range(2))
-        nmap = torch.empty((3, H, W), dtype=torch.float32, device=means3D.device)
-        color, radii = _RasterizeGaussians._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales,
-                                                rotations, cov3Ds_precomp, rs, maps, (nrm_in, nmap))
-        ctx.cam_shapes = (viewmatrix.shape, projmatrix.shape, campos.shape)
-        return color, radii, maps[0], maps[1], nmap
-
-    @staticmethod
-    def backward(ctx, grad_out_color, _, grad_depth, grad_alpha, grad_normal):
-        need = tuple(ctx.needs_input_grad[9:12])
-        means3D = ctx.saved_tensors[0]
-        cam = _CameraGrads(1, means3D.shape[0], means3D.device, need) if any(need) else None
-        ab = _abs_output(ctx, means3D.device)
-        if grad_normal is None:
-            g = _RasterizeGaussians._bwd(ctx, grad_out_color, grad_depth, grad_alpha, cam, abs_out=ab) + (None,)
-        else:
-            g = _RasterizeGaussians._bwd(ctx, grad_out_color, grad_depth, grad_alpha, cam,
-                                         (grad_normal, ctx.needs_input_grad[8]), abs_out=ab)
-        return g[:8] + g[9:] + (cam.grads(ctx.cam_shapes) if cam else (None, None, None)) + (None, ab)
-
-
-def _surface_grads(ctx, grad_depth, grad_alpha, grad_median, grad_dist, grad_normal):
-    """Common part of the surface Functions' backward: the (nrm, surf) arguments of `_bwd`, each None when the loss
-    does not use those maps."""
-    nrm = None if grad_normal is None else (grad_normal, ctx.needs_input_grad[8])
-    surf = None
-    if grad_median is not None or grad_dist is not None:
-        surf = (ctx.near, ctx.far, grad_median, grad_dist)
-    return nrm, surf
-
-
-class _RasterizeGaussiansSurface(torch.autograd.Function):
-    """`_RasterizeGaussiansDepthAlpha` + the median-depth and distortion maps [1,H,W] (and, with `normals` [P,3],
-    the normal map of `_RasterizeGaussiansNormal`), with the camera as explicit inputs (pass detached tensors for no
-    camera gradient).  Gradients are not materialised: a map the loss does not use reaches the library as NULL, and a
-    loss that uses neither surface map runs the normal / depth-alpha / colour-only backward."""
-
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, normals,
-                viewmatrix, projmatrix, campos, raster_settings, near, far, means2D_abs=None):
-        ctx.set_materialize_grads(False)
-        _abs_input(ctx, means2D_abs, (means3D.shape[0], 3))
-        rs = raster_settings._replace(viewmatrix=viewmatrix.detach(), projmatrix=projmatrix.detach(),
-                                      campos=campos.detach())
-        H, W = int(rs.image_height), int(rs.image_width)
-        dev = means3D.device
-        nrm = None
-        if normals is not None:
-            nrm_in = _f32c(normals, "normals")
-            if nrm_in is None or nrm_in.shape != (means3D.shape[0], 3):
-                raise ValueError("normals must have dimensions (num_points, 3)")
-            nrm = (nrm_in, torch.empty((3, H, W), dtype=torch.float32, device=dev))
-        maps = tuple(torch.empty((1, H, W), dtype=torch.float32, device=dev) for _ in range(4))
-        color, radii = _RasterizeGaussians._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales,
-                                                rotations, cov3Ds_precomp, rs, maps[:2], nrm,
-                                                (near, far, maps[2], maps[3]))
-        ctx.cam_shapes = (viewmatrix.shape, projmatrix.shape, campos.shape)
-        ctx.near, ctx.far = near, far
-        return (color, radii) + maps + ((nrm[1],) if nrm is not None else ())
-
-    @staticmethod
-    def backward(ctx, grad_out_color, _, grad_depth, grad_alpha, grad_median, grad_dist, grad_normal=None):
-        need = tuple(ctx.needs_input_grad[9:12])
-        means3D = ctx.saved_tensors[0]
-        cam = _CameraGrads(1, means3D.shape[0], means3D.device, need) if any(need) else None
-        nrm, surf = _surface_grads(ctx, grad_depth, grad_alpha, grad_median, grad_dist, grad_normal)
-        ab = _abs_output(ctx, means3D.device)
-        g = _RasterizeGaussians._bwd(ctx, grad_out_color, grad_depth, grad_alpha, cam, nrm, surf, ab)
-        if nrm is None:
-            g = g + (None,)
-        return g[:8] + g[9:] + (cam.grads(ctx.cam_shapes) if cam else (None, None, None)) + (None, None, None, ab)
 
 
 _N_STREAMS = int(os.environ.get("DGMESH_B200_STREAMS", "2"))
@@ -651,19 +508,19 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings):
         return _RasterizeGaussiansBatch._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                             cov3Ds_precomp, settings, None)
+                                             cov3Ds_precomp, settings)
 
     @staticmethod
     def backward(ctx, grad_out_color, _):
-        return _RasterizeGaussiansBatch._bwd(ctx, grad_out_color, None, None)
+        return _RasterizeGaussiansBatch._bwd(ctx, grad_out_color)   # its last entry, dL/dnormals, is None here
 
     @staticmethod
     def _fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings,
-             maps, cams=None, nrm=None, surf=None, saved=()):
+             maps=None, nrm=None, surf=None, cams=None, saved=()):
         """maps: None (colour only) or the (depth, alpha) [F,1,H,W] tensors the forward writes as well.
-        cams: None (the settings' cameras), or the stacked (views [F,4,4], projs [F,4,4], campos [F,3]) to use.
         nrm: None, or (normals [P,3] shared or [F,P,3] per frame, normal maps [F,3,H,W]) (with maps).
         surf: None, or (near, far, median [F,1,H,W], distortion [F,1,H,W]) (with maps).
+        cams: None (the settings' cameras), or the stacked (views [F,4,4], projs [F,4,4], campos [F,3]) to use.
         saved: more tensors to save for the backward, after (means3D, radii)."""
         rs0 = settings[0]
         F = len(settings)
@@ -701,7 +558,6 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
         H, W = int(rs0.image_height), int(rs0.image_width)
         M = int(sh_.shape[-2]) if sh_ is not None else 0
         key = (dev.index, W, H)
-        lib = _dgm_lib.lib()
         p = _dgm_lib.ptr
         first = []
 
@@ -719,23 +575,13 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
             tail = (ws.geom, ws.gs, ws.binning, ws.bs, R_cap, ws.img, ws.is_, ws.status,
                     notify.host_ptr if notify else None, notify.event if notify else None, lo, hi, int(mt),
                     _N_STREAMS, _dgm_lib.stream_ptr())
-            if surf is not None:
-                n_in, n_map = nrm if nrm is not None else (None, None)
-                _dgm_lib.check(lib.dgr_forward_batch_surf(*head, p(maps[0]), p(maps[1]), p(n_in),
-                                                          int(n_in is not None and n_in.ndim == 3), p(n_map),
-                                                          ws.nrm.data_ptr() if nrm is not None else None,
-                                                          ws.nrm_stride, float(surf[0]), float(surf[1]), p(surf[2]),
-                                                          p(surf[3]), ws.surf.data_ptr(), ws.surf_stride, *tail),
-                               "dgr_forward_batch_surf")
-            elif nrm is not None:
-                _dgm_lib.check(lib.dgr_forward_batch_nrm(*head, p(maps[0]), p(maps[1]), p(nrm[0]),
-                                                         int(nrm[0].ndim == 3), p(nrm[1]), ws.nrm.data_ptr(),
-                                                         ws.nrm_stride, *tail), "dgr_forward_batch_nrm")
-            elif maps is None:
-                _dgm_lib.check(lib.dgr_forward_batch(*head, *tail), "dgr_forward_batch")
-            else:
-                _dgm_lib.check(lib.dgr_forward_batch_aux(*head, p(maps[0]), p(maps[1]), *tail),
-                               "dgr_forward_batch_aux")
+            _enqueue("dgr_forward_batch", (
+                (None, head), ("_aux", None if maps is None else (p(maps[0]), p(maps[1]))),
+                ("_nrm", None if nrm is None else (p(nrm[0]), int(nrm[0].ndim == 3), p(nrm[1]), ws.nrm.data_ptr(),
+                                                   ws.nrm_stride)),
+                ("_surf", None if surf is None else (float(surf[0]), float(surf[1]), p(surf[2]), p(surf[3]),
+                                                     ws.surf.data_ptr(), ws.surf_stride)),
+                (None, tail)))
             return color, radii, ws
 
         (color, radii, ws), _ = _run_sized(run, key, P, dev.index, F)
@@ -748,13 +594,9 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
         return color, radii
 
     @staticmethod
-    def _bwd(ctx, grad_out_color, grad_depth, grad_alpha, cam=None, nrm=None, surf=None, abs_out=None):
-        """cam: None, or the _CameraGrads the backward writes the camera gradients to.
-        nrm: None, or (upstream gradient of the normal maps, whether dL/dnormals is needed); then the result has a
-        tenth entry, dL/dnormals ([F,P,3] for per-frame normals, else [P,3]; or None).
-        surf: None, or (near, far, upstream gradients of the median-depth and distortion maps, each None when
-        unused, not both).
-        abs_out: None, or the [F,P,3] tensor the backward writes the absolute screen-space gradients to."""
+    def _bwd(ctx, grad_out_color, grad_depth=None, grad_alpha=None, cam=None, nrm=None, surf=None, abs_out=None):
+        """As _RasterizeGaussians._bwd for F frames: the upstream gradients have a leading F dimension, abs_out is
+        [F,P,3], and dL/dnormals is [F,P,3] for per-frame normals, else [P,3]."""
         bg, sh, col, opac, sc, rot, cov = ctx.tensors
         views, projs, cams, tx, ty = ctx.cams
         means3D, radii = ctx.saved_tensors[:2]
@@ -795,174 +637,29 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
         head = (F, P, rs0.sh_degree, M, p(bg), W, H, p(means3D), p(sh), p(col), p(sc), float(rs0.scale_modifier),
                 p(rot), p(cov), pf, p(views), p(projs), p(cams), tx, ty, p(radii), ws.geom, ws.gs, ws.binning, ws.bs,
                 ws.R_cap, ws.img, ws.is_, p(dpix))
-        tail = (ptrs[0], ptrs[1], ptrs[2] if col is not None else None, ptrs[3], ptrs[4] if cov is not None else None,
-                ptrs[7] if M else None, ptrs[5], ptrs[6], _N_STREAMS, _dgm_lib.stream_ptr())
-        lib = _dgm_lib.lib()
-        dnormals = None
-        if surf is not None or abs_out is not None:
-            gd, ga = _f32c(grad_depth, "grad_depth"), _f32c(grad_alpha, "grad_alpha")
-            gn = _f32c(nrm[0], "grad_normal") if nrm is not None else None
-            npf = ctx.normals_pf
-            if nrm is not None and nrm[1]:
-                dnormals = torch.empty((F, P, 3) if npf else (P, 3), dtype=torch.float32, device=means3D.device)
-            cargs = cam.args() if cam is not None else (None, None, None, None, 0)
-            sargs = (0.0, 0.0, None, None, None, 0)
-            if surf is not None:
-                sargs = (float(surf[0]), float(surf[1]), p(_f32c(surf[2], "grad_median_depth")),
-                         p(_f32c(surf[3], "grad_distortion")), ws.surf.data_ptr(), ws.surf_stride)
-            _dgm_lib.check(lib.dgr_backward_batch_abs(*head, p(gd), p(ga), *tail[:-2], *cargs, p(gn), npf,
-                                                      p(dnormals), ws.nrm.data_ptr() if gn is not None else None,
-                                                      ws.nrm_stride, *sargs, p(abs_out), *tail[-2:]),
-                           "dgr_backward_batch_abs")
-        elif nrm is not None:
-            gd, ga, gn = _f32c(grad_depth, "grad_depth"), _f32c(grad_alpha, "grad_alpha"), _f32c(nrm[0], "grad_normal")
+        grads = (ptrs[0], ptrs[1], ptrs[2] if col is not None else None, ptrs[3], ptrs[4] if cov is not None else None,
+                 ptrs[7] if M else None, ptrs[5], ptrs[6])
+        aux = nrm_args = surf_args = dnormals = None
+        if grad_depth is not None or grad_alpha is not None:
+            aux = (p(_f32c(grad_depth, "grad_depth")), p(_f32c(grad_alpha, "grad_alpha")))
+        if nrm is not None:
             npf = ctx.normals_pf
             if nrm[1]:
                 dnormals = torch.empty((F, P, 3) if npf else (P, 3), dtype=torch.float32, device=means3D.device)
-            cargs = cam.args() if cam is not None else (None, None, None, None, 0)
-            _dgm_lib.check(lib.dgr_backward_batch_nrm(*head, p(gd), p(ga), *tail[:-2], *cargs, p(gn), npf,
-                                                      p(dnormals), ws.nrm.data_ptr(), ws.nrm_stride, *tail[-2:]),
-                           "dgr_backward_batch_nrm")
-        elif cam is not None:
-            gd, ga = _f32c(grad_depth, "grad_depth"), _f32c(grad_alpha, "grad_alpha")
-            _dgm_lib.check(lib.dgr_backward_batch_cam(*head, p(gd), p(ga), *tail[:-2], *cam.args(), *tail[-2:]),
-                           "dgr_backward_batch_cam")
-        elif grad_depth is None and grad_alpha is None:
-            _dgm_lib.check(lib.dgr_backward_batch(*head, *tail), "dgr_backward_batch")
-        else:
-            gd, ga = _f32c(grad_depth, "grad_depth"), _f32c(grad_alpha, "grad_alpha")
-            _dgm_lib.check(lib.dgr_backward_batch_aux(*head, p(gd), p(ga), *tail), "dgr_backward_batch_aux")
-        g = (gview(3, _PF_MEANS, P, 3), gview(0, 0, F, P, 3) if ctx.has_m2d else None,
-             gview(7, _PF_COLOR, P, M, 3) if sh is not None else None,
-             gview(2, _PF_COLOR, P, 3) if col is not None else None,
-             gview(1, _PF_OPAC, P, 1), gview(5, _PF_SCALES, P, 3) if sc is not None else None,
-             gview(6, _PF_ROTS, P, 4) if rot is not None else None,
-             gview(4, _PF_COV, P, 6) if cov is not None else None, None)
-        return g if nrm is None else g + (dnormals,)
-
-
-class _RasterizeGaussiansBatchDepthAlpha(torch.autograd.Function):
-    """`_RasterizeGaussiansBatch` + the depth and alpha maps [F,1,H,W] (see _RasterizeGaussiansDepthAlpha)."""
-
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings):
-        ctx.set_materialize_grads(False)
-        F, H, W = len(settings), int(settings[0].image_height), int(settings[0].image_width)
-        maps = tuple(torch.empty((F, 1, H, W), dtype=torch.float32, device=means3D.device) for _ in range(2))
-        color, radii = _RasterizeGaussiansBatch._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales,
-                                                     rotations, cov3Ds_precomp, settings, maps)
-        return color, radii, maps[0], maps[1]
-
-    @staticmethod
-    def backward(ctx, grad_out_color, _, grad_depth, grad_alpha):
-        return _RasterizeGaussiansBatch._bwd(ctx, grad_out_color, grad_depth, grad_alpha)
-
-
-class _RasterizeGaussiansBatchCam(torch.autograd.Function):
-    """`_RasterizeGaussiansBatch` (depth_alpha: + the maps) with the frames' cameras as explicit inputs: views
-    [F,4,4], projs [F,4,4] and campos [F,3] replace the settings' tensors and receive gradients (see
-    _RasterizeGaussiansCam)."""
-
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, views, projs,
-                campos, settings, depth_alpha, means2D_abs=None):
-        ctx.set_materialize_grads(False)
-        _abs_input(ctx, means2D_abs, (len(settings), means3D.shape[-2], 3))
-        maps = None
-        if depth_alpha:
-            F, H, W = len(settings), int(settings[0].image_height), int(settings[0].image_width)
-            maps = tuple(torch.empty((F, 1, H, W), dtype=torch.float32, device=means3D.device) for _ in range(2))
-        color, radii = _RasterizeGaussiansBatch._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales,
-                                                     rotations, cov3Ds_precomp, settings, maps, (views, projs, campos))
-        ctx.cam_shapes = (views.shape, projs.shape, campos.shape)
-        return (color, radii) + (maps if depth_alpha else ())
-
-    @staticmethod
-    def backward(ctx, grad_out_color, _, grad_depth=None, grad_alpha=None):
-        need = tuple(ctx.needs_input_grad[8:11])
-        means3D = ctx.saved_tensors[0]
-        cam = _CameraGrads(ctx.ws.F, means3D.shape[-2], means3D.device, need) if any(need) else None
-        ab = _abs_output(ctx, means3D.device)
-        g = _RasterizeGaussiansBatch._bwd(ctx, grad_out_color, grad_depth, grad_alpha, cam, abs_out=ab)
-        return g[:8] + (cam.grads(ctx.cam_shapes) if cam else (None, None, None)) + (None, None, ab)
-
-
-class _RasterizeGaussiansBatchNormal(torch.autograd.Function):
-    """`_RasterizeGaussiansBatchDepthAlpha` + the normal maps [F,3,H,W] of `normals` ([P,3] shared by the frames or
-    [F,P,3] per frame), optionally with the frames' cameras as explicit inputs (views / projs / campos None: the
-    settings' cameras, no camera gradient).  See _RasterizeGaussiansNormal."""
-
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, normals, views,
-                projs, campos, settings, means2D_abs=None):
-        ctx.set_materialize_grads(False)
-        _abs_input(ctx, means2D_abs, (len(settings), means3D.shape[-2], 3))
-        F, H, W = len(settings), int(settings[0].image_height), int(settings[0].image_width)
-        nrm_in = _f32c(normals, "normals")
-        P = means3D.shape[-2]
-        if nrm_in is None or nrm_in.shape not in ((P, 3), (F, P, 3)):
-            raise ValueError("normals must have dimensions (num_points, 3) or (num_frames, num_points, 3)")
-        maps = tuple(torch.empty((F, 1, H, W), dtype=torch.float32, device=means3D.device) for _ in range(2))
-        nmap = torch.empty((F, 3, H, W), dtype=torch.float32, device=means3D.device)
-        cams = None if views is None else (views, projs, campos)
-        color, radii = _RasterizeGaussiansBatch._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales,
-                                                     rotations, cov3Ds_precomp, settings, maps, cams, (nrm_in, nmap))
-        ctx.cam_shapes = None if views is None else (views.shape, projs.shape, campos.shape)
-        return color, radii, maps[0], maps[1], nmap
-
-    @staticmethod
-    def backward(ctx, grad_out_color, _, grad_depth, grad_alpha, grad_normal):
-        need = tuple(ctx.needs_input_grad[9:12])
-        means3D = ctx.saved_tensors[0]
-        cam = _CameraGrads(ctx.ws.F, means3D.shape[-2], means3D.device, need) if any(need) else None
-        ab = _abs_output(ctx, means3D.device)
-        if grad_normal is None:
-            g = _RasterizeGaussiansBatch._bwd(ctx, grad_out_color, grad_depth, grad_alpha, cam, abs_out=ab) + (None,)
-        else:
-            g = _RasterizeGaussiansBatch._bwd(ctx, grad_out_color, grad_depth, grad_alpha, cam,
-                                              (grad_normal, ctx.needs_input_grad[8]), abs_out=ab)
-        return g[:8] + g[9:] + (cam.grads(ctx.cam_shapes) if cam else (None, None, None)) + (None, ab)
-
-
-class _RasterizeGaussiansBatchSurface(torch.autograd.Function):
-    """`_RasterizeGaussiansBatchDepthAlpha` + the median-depth and distortion maps [F,1,H,W] (and, with `normals`
-    [P,3] or [F,P,3], the normal maps of `_RasterizeGaussiansBatchNormal`), optionally with the frames' cameras as
-    explicit inputs (views / projs / campos None: the settings' cameras).  See _RasterizeGaussiansSurface."""
-
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, normals, views,
-                projs, campos, settings, near, far, means2D_abs=None):
-        ctx.set_materialize_grads(False)
-        _abs_input(ctx, means2D_abs, (len(settings), means3D.shape[-2], 3))
-        F, H, W = len(settings), int(settings[0].image_height), int(settings[0].image_width)
-        dev = means3D.device
-        nrm = None
-        if normals is not None:
-            nrm_in = _f32c(normals, "normals")
-            P = means3D.shape[-2]
-            if nrm_in is None or nrm_in.shape not in ((P, 3), (F, P, 3)):
-                raise ValueError("normals must have dimensions (num_points, 3) or (num_frames, num_points, 3)")
-            nrm = (nrm_in, torch.empty((F, 3, H, W), dtype=torch.float32, device=dev))
-        maps = tuple(torch.empty((F, 1, H, W), dtype=torch.float32, device=dev) for _ in range(4))
-        cams = None if views is None else (views, projs, campos)
-        color, radii = _RasterizeGaussiansBatch._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales,
-                                                     rotations, cov3Ds_precomp, settings, maps[:2], cams, nrm,
-                                                     (near, far, maps[2], maps[3]))
-        ctx.cam_shapes = None if views is None else (views.shape, projs.shape, campos.shape)
-        ctx.near, ctx.far = near, far
-        return (color, radii) + maps + ((nrm[1],) if nrm is not None else ())
-
-    @staticmethod
-    def backward(ctx, grad_out_color, _, grad_depth, grad_alpha, grad_median, grad_dist, grad_normal=None):
-        need = tuple(ctx.needs_input_grad[9:12])
-        means3D = ctx.saved_tensors[0]
-        cam = _CameraGrads(ctx.ws.F, means3D.shape[-2], means3D.device, need) if any(need) else None
-        nrm, surf = _surface_grads(ctx, grad_depth, grad_alpha, grad_median, grad_dist, grad_normal)
-        ab = _abs_output(ctx, means3D.device)
-        g = _RasterizeGaussiansBatch._bwd(ctx, grad_out_color, grad_depth, grad_alpha, cam, nrm, surf, ab)
-        if nrm is None:
-            g = g + (None,)
-        return g[:8] + g[9:] + (cam.grads(ctx.cam_shapes) if cam else (None, None, None)) + (None, None, None, ab)
+            nrm_args = (p(_f32c(nrm[0], "grad_normal")), npf, p(dnormals), ws.nrm.data_ptr(), ws.nrm_stride)
+        if surf is not None:
+            surf_args = (float(surf[0]), float(surf[1]), p(_f32c(surf[2], "grad_median_depth")),
+                         p(_f32c(surf[3], "grad_distortion")), ws.surf.data_ptr(), ws.surf_stride)
+        _enqueue("dgr_backward_batch", ((None, head), ("_aux", aux), (None, grads),
+                                        ("_cam", None if cam is None else cam.args()), ("_nrm", nrm_args),
+                                        ("_surf", surf_args), ("_abs", None if abs_out is None else (p(abs_out),)),
+                                        (None, (_N_STREAMS, _dgm_lib.stream_ptr()))))
+        return (gview(3, _PF_MEANS, P, 3), gview(0, 0, F, P, 3) if ctx.has_m2d else None,
+                gview(7, _PF_COLOR, P, M, 3) if sh is not None else None,
+                gview(2, _PF_COLOR, P, 3) if col is not None else None,
+                gview(1, _PF_OPAC, P, 1), gview(5, _PF_SCALES, P, 3) if sc is not None else None,
+                gview(6, _PF_ROTS, P, 4) if rot is not None else None,
+                gview(4, _PF_COV, P, 6) if cov is not None else None, dnormals)
 
 
 _MAX_FEATURES = 64
@@ -1021,103 +718,109 @@ def _features_bwd(ws, st, W, H, fmap, grad, need):
     return dfeat
 
 
-class _RasterizeGaussiansFeatures(torch.autograd.Function):
-    """`_RasterizeGaussiansDepthAlpha` + the feature map sum_i f_i alpha_i T_i [C,H,W] of `features` [P,C], with the
-    camera as explicit inputs (pass detached tensors for no camera gradient).  The map is a pass over the forward's
-    workspaces (dgr_features_fwd); its backward (dgr_features_bwd) runs before the rasterizer backward, which carries
-    it to every input.  Gradients are not materialised: a loss that does not use the feature map runs exactly the
-    depth / alpha (or colour-only) backward."""
+def _check_normals(normals, P, F=None):
+    """normals as a float32 CUDA tensor [P,3] (or, with F, [P,3] shared by the frames or [F,P,3] per frame)."""
+    n = _f32c(normals, "normals")
+    if F is None:
+        if n is None or n.shape != (P, 3):
+            raise ValueError("normals must have dimensions (num_points, 3)")
+    elif n is None or n.shape not in ((P, 3), (F, P, 3)):
+        raise ValueError("normals must have dimensions (num_points, 3) or (num_frames, num_points, 3)")
+    return n
 
-    @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, features,
-                viewmatrix, projmatrix, campos, raster_settings):
-        ctx.set_materialize_grads(False)
-        rs = raster_settings._replace(viewmatrix=viewmatrix.detach(), projmatrix=projmatrix.detach(),
-                                      campos=campos.detach())
-        H, W = int(rs.image_height), int(rs.image_width)
-        dev = means3D.device
-        st = _FeatureState(_check_features(features, means3D.shape[0]), 1, dev)
-        maps = tuple(torch.empty((1, H, W), dtype=torch.float32, device=dev) for _ in range(2))
-        fmap = torch.empty((st.C, H, W), dtype=torch.float32, device=dev)
-        color, radii = _RasterizeGaussians._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales,
-                                                rotations, cov3Ds_precomp, rs, maps, saved=(fmap,))
+
+# the outputs of the maps Functions, in order; a map the request does not ask for is None
+_MAPS = ("color", "radii", "depth", "alpha", "median_depth", "distortion", "normal", "features")
+
+
+def _maps_forward(ctx, batch, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                  normals, features, viewmatrix, projmatrix, campos, means2D_abs, settings, request):
+    """Forward of the maps Functions (F frames when `batch`): the outputs of _MAPS."""
+    ctx.set_materialize_grads(False)
+    depth_alpha, surface = request
+    F = len(settings) if batch else None
+    lead = (F,) if batch else ()
+    rs0 = settings[0] if batch else settings
+    H, W = int(rs0.image_height), int(rs0.image_width)
+    P, dev = means3D.shape[-2], means3D.device
+
+    def new_map(channels):
+        return torch.empty(lead + (channels, H, W), dtype=torch.float32, device=dev)
+
+    ctx.abs_shape = lead + (P, 3)
+    if means2D_abs is not None and tuple(means2D_abs.shape) != ctx.abs_shape:
+        raise ValueError(f"means2D_abs must have dimensions {ctx.abs_shape}")
+    maps = (new_map(1), new_map(1)) if depth_alpha else None
+    nrm = None if normals is None else (_check_normals(normals, P, F), new_map(3))
+    surf = None if surface is None else (surface[0], surface[1], new_map(1), new_map(1))
+    st = fmap = None
+    if features is not None:
+        st = _FeatureState(_check_features(features, P, F), F or 1, dev)
+        fmap = new_map(st.C)
+    cams = None if viewmatrix is None else (viewmatrix, projmatrix, campos)
+    core = _RasterizeGaussiansBatch if batch else _RasterizeGaussians
+    color, radii = core._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                             settings, maps, nrm, surf, cams, () if fmap is None else (fmap,))
+    if st is not None:
         _features_fwd(ctx.ws, st, W, H, fmap)
-        ctx.feat = st
-        ctx.cam_shapes = (viewmatrix.shape, projmatrix.shape, campos.shape)
-        return color, radii, maps[0], maps[1], fmap
+    ctx.feat, ctx.surface, ctx.frames = st, surface, F or 1
+    ctx.cam_shapes = None if cams is None else tuple(t.shape for t in cams)
+    return (color, radii) + (maps or (None, None)) + (surf[2:] if surf else (None, None)) + \
+        (None if nrm is None else nrm[1], fmap)
+
+
+def _maps_backward(ctx, core, grad_color, _, grad_depth, grad_alpha, grad_median, grad_dist, grad_normal,
+                   grad_features):
+    """Backward of the maps Functions: the feature pass first (it adds to the forward's accumulators), then `core`'s
+    rasterizer backward with the segments the upstream gradients use."""
+    *_, need_normals, need_features, need_view, need_proj, need_campos, need_abs, _, _ = ctx.needs_input_grad
+    means3D = ctx.saved_tensors[0]
+    dfeat = None
+    if grad_features is not None:
+        fmap = ctx.saved_tensors[2]
+        dfeat = _features_bwd(ctx.ws, ctx.feat, fmap.shape[-1], fmap.shape[-2], fmap, grad_features, need_features)
+    need = (need_view, need_proj, need_campos)
+    cam = _CameraGrads(ctx.frames, means3D.shape[-2], means3D.device, need) if any(need) else None
+    ab = torch.empty(ctx.abs_shape, dtype=torch.float32, device=means3D.device) if need_abs else None
+    nrm = None if grad_normal is None else (grad_normal, need_normals)
+    surf = None if grad_median is None and grad_dist is None else (*ctx.surface, grad_median, grad_dist)
+    g = core._bwd(ctx, grad_color, grad_depth, grad_alpha, cam, nrm, surf, ab)
+    return g + (dfeat,) + (cam.grads(ctx.cam_shapes) if cam else (None, None, None)) + (ab, None, None)
+
+
+class _RasterizeGaussiansMaps(torch.autograd.Function):
+    """`_RasterizeGaussians` + the maps a request asks for.  Inputs: the eight Gaussian tensors of
+    `_RasterizeGaussians`; normals [P,3] for the normal map sum_i n_i alpha_i T_i [3,H,W] and features [P,C] for the
+    feature map [C,H,W] (each None when not asked for); viewmatrix [4,4], projmatrix [4,4] and campos [3], which
+    replace the settings' tensors and receive gradients (None: the settings' camera, no camera gradient);
+    means2D_abs [P,3], whose gradient is the absolute screen-space gradient (or None); the settings; the request
+    (depth_alpha: the depth map sum_i d_i alpha_i T_i and the alpha map 1 - T_final [1,H,W]; (near, far) for the
+    median-depth and distortion maps [1,H,W], or None).  Outputs: _MAPS.  Normals, surface maps and features need
+    depth_alpha; the feature map is a pass over the forward's workspaces (dgr_features_fwd / _bwd).  Gradients are
+    not materialised: a map the loss does not use reaches the library as NULL, and the backward calls the narrowest
+    entry point the loss needs."""
 
     @staticmethod
-    def backward(ctx, grad_out_color, _, grad_depth, grad_alpha, grad_features):
-        need = tuple(ctx.needs_input_grad[9:12])
-        means3D = ctx.saved_tensors[0]
-        H, W = int(ctx.raster_settings.image_height), int(ctx.raster_settings.image_width)
-        dfeat = None
-        if grad_features is not None:
-            dfeat = _features_bwd(ctx.ws, ctx.feat, W, H, ctx.saved_tensors[2], grad_features,
-                                  ctx.needs_input_grad[8])
-        cam = _CameraGrads(1, means3D.shape[0], means3D.device, need) if any(need) else None
-        g = _RasterizeGaussians._bwd(ctx, grad_out_color, grad_depth, grad_alpha, cam)
-        return g[:8] + (dfeat,) + (cam.grads(ctx.cam_shapes) if cam else (None, None, None)) + (None,)
-
-
-class _RasterizeGaussiansBatchFeatures(torch.autograd.Function):
-    """`_RasterizeGaussiansBatchDepthAlpha` + the feature maps [F,C,H,W] of `features` ([P,C] shared by the frames,
-    its gradient the sum over the frames, or [F,P,C] per frame), optionally with the normal maps (`normals`), the
-    surface maps (`surface` = (near, far)) and the frames' cameras as explicit inputs (views / projs / campos None:
-    the settings' cameras).  Outputs: color, radii, depth, alpha, features[, median_depth, distortion][, normal].
-    See _RasterizeGaussiansFeatures."""
+    def forward(ctx, *inputs):
+        return _maps_forward(ctx, False, *inputs)
 
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, features,
-                normals, views, projs, campos, settings, surface):
-        ctx.set_materialize_grads(False)
-        F, H, W = len(settings), int(settings[0].image_height), int(settings[0].image_width)
-        dev = means3D.device
-        P = means3D.shape[-2]
-        st = _FeatureState(_check_features(features, P, F), F, dev)
-        nrm = None
-        if normals is not None:
-            nrm_in = _f32c(normals, "normals")
-            if nrm_in is None or nrm_in.shape not in ((P, 3), (F, P, 3)):
-                raise ValueError("normals must have dimensions (num_points, 3) or (num_frames, num_points, 3)")
-            nrm = (nrm_in, torch.empty((F, 3, H, W), dtype=torch.float32, device=dev))
-        maps = tuple(torch.empty((F, 1, H, W), dtype=torch.float32, device=dev) for _ in range(4 if surface else 2))
-        surf = (surface[0], surface[1], maps[2], maps[3]) if surface else None
-        fmap = torch.empty((F, st.C, H, W), dtype=torch.float32, device=dev)
-        cams = None if views is None else (views, projs, campos)
-        color, radii = _RasterizeGaussiansBatch._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales,
-                                                     rotations, cov3Ds_precomp, settings, maps[:2], cams, nrm, surf,
-                                                     saved=(fmap,))
-        _features_fwd(ctx.ws, st, W, H, fmap)
-        ctx.feat = st
-        ctx.cam_shapes = None if views is None else (views.shape, projs.shape, campos.shape)
-        if surface:
-            ctx.near, ctx.far = surface
-        ctx.n_out = (surface is not None, nrm is not None)
-        return (color, radii, maps[0], maps[1], fmap) + maps[2:] + ((nrm[1],) if nrm is not None else ())
+    def backward(ctx, *grads):
+        return _maps_backward(ctx, _RasterizeGaussians, *grads)
+
+
+class _RasterizeGaussiansBatchMaps(torch.autograd.Function):
+    """`_RasterizeGaussiansMaps` for F frames over `_RasterizeGaussiansBatch`: the settings are a tuple, every map
+    has a leading F dimension, normals and features are [P,.] shared by the frames (their gradient the sum over the
+    frames) or [F,P,.] per frame, the cameras [F,4,4], [F,4,4], [F,3] and means2D_abs [F,P,3]."""
 
     @staticmethod
-    def backward(ctx, grad_out_color, _, grad_depth, grad_alpha, grad_features, *rest):
-        has_surf, has_nrm = ctx.n_out
-        grad_median, grad_dist = rest[:2] if has_surf else (None, None)
-        grad_normal = rest[-1] if has_nrm else None
-        need = tuple(ctx.needs_input_grad[10:13])
-        means3D = ctx.saved_tensors[0]
-        rs0 = ctx.settings[0]
-        H, W = int(rs0.image_height), int(rs0.image_width)
-        dfeat = None
-        if grad_features is not None:
-            dfeat = _features_bwd(ctx.ws, ctx.feat, W, H, ctx.saved_tensors[2], grad_features,
-                                  ctx.needs_input_grad[8])
-        cam = _CameraGrads(ctx.ws.F, means3D.shape[-2], means3D.device, need) if any(need) else None
-        nrm = None if grad_normal is None else (grad_normal, ctx.needs_input_grad[9])
-        surf = None
-        if grad_median is not None or grad_dist is not None:
-            surf = (ctx.near, ctx.far, grad_median, grad_dist)
-        g = _RasterizeGaussiansBatch._bwd(ctx, grad_out_color, grad_depth, grad_alpha, cam, nrm, surf)
-        dnormals = g[9] if nrm is not None else None
-        return (g[:8] + (dfeat, dnormals) + (cam.grads(ctx.cam_shapes) if cam else (None, None, None)) +
-                (None, None))
+    def forward(ctx, *inputs):
+        return _maps_forward(ctx, True, *inputs)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        return _maps_backward(ctx, _RasterizeGaussiansBatch, *grads)
 
 
 def rasterize_gaussians_batch(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
@@ -1137,6 +840,24 @@ def _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp):
     return tuple(e if x is None else x for x in (shs, colors_precomp, scales, rotations, cov3D_precomp))
 
 
+def _request_maps(plain, function, settings, cams, means3D, means2D, opacities, shs, colors_precomp, scales,
+                  rotations, cov3D_precomp, depth_alpha, normals, surface, features, means2D_abs):
+    """The rasterizers' `_maps`: the reference-shaped `plain` Function when only colour is asked for, else the maps
+    `function`; the outputs by name, in _MAPS order, without the maps not asked for."""
+    if features is not None and means2D_abs is not None:
+        # the feature pass adds its dL/dalpha in a pass of its own, so no per-pixel total exists to take |.| of
+        raise ValueError("abs_grad: the absolute screen-space gradient is not available with feature or flow maps")
+    sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
+    depth_alpha = bool(depth_alpha) or normals is not None or surface is not None or features is not None
+    if not depth_alpha and cams[0] is None and means2D_abs is None:
+        color, radii = plain.apply(means3D, means2D, sh, col, opacities, sc, rot, cov, settings)
+        return {"color": color, "radii": radii}
+    surface = None if surface is None else (float(surface[0]), float(surface[1]))
+    out = function.apply(means3D, means2D, sh, col, opacities, sc, rot, cov, normals, features, *cams, means2D_abs,
+                         settings, (depth_alpha, surface))
+    return {name: t for name, t in zip(_MAPS, out) if t is not None}
+
+
 class BatchGaussianRasterizer(nn.Module):
     """`GaussianRasterizer` for a batch of frames (one settings tuple per frame, same image size)."""
 
@@ -1149,8 +870,8 @@ class BatchGaussianRasterizer(nn.Module):
         """F frames -> (color [F,3,H,W], radii [F,P]).  means2D_abs ([F,P,3], e.g. zeros with requires_grad) receives
         in its .grad each frame's absolute screen-space gradient (see GaussianRasterizer.forward_abs_grad)."""
         if means2D_abs is not None:
-            return self._abs_grad(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
-                                  False, means2D_abs)
+            return tuple(self._maps(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                                    means2D_abs=means2D_abs).values())
         if (shs is None) == (colors_precomp is None):
             raise Exception('Please provide excatly one of either SHs or precomputed colors!')
         if ((scales is None or rotations is None) and cov3D_precomp is None) or \
@@ -1162,17 +883,28 @@ class BatchGaussianRasterizer(nn.Module):
                                          e if scales is None else scales, e if rotations is None else rotations,
                                          e if cov3D_precomp is None else cov3D_precomp, self.settings)
 
+    def _maps(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
+              cov3D_precomp=None, depth_alpha=False, normals=None, surface=None, features=None, camera_grad=False,
+              means2D_abs=None):
+        """Every frame's outputs by name, in _MAPS order: "color" and "radii"; "depth" and "alpha" with depth_alpha
+        or any other map; "median_depth" and "distortion" with surface = (near, far); "normal" with normals ([P,3]
+        or [F,P,3]); "features" with features ([P,C] or [F,P,C]).  camera_grad: the frames' camera tensors receive
+        gradients.  means2D_abs: see `forward` (not with features)."""
+        cams = (None, None, None)
+        if camera_grad:
+            cams = tuple(torch.stack([getattr(s, k) for s in self.settings])
+                         for k in ("viewmatrix", "projmatrix", "campos"))
+        return _request_maps(_RasterizeGaussiansBatch, _RasterizeGaussiansBatchMaps, self.settings, cams, means3D,
+                             means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp, depth_alpha,
+                             normals, surface, features, means2D_abs)
+
     def forward_depth_alpha(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None,
                             rotations=None, cov3D_precomp=None, means2D_abs=None):
         """`forward` + the depth map sum_i d_i alpha_i T_i (view-space depth, unnormalised: expected depth is
         depth / alpha) and the alpha map 1 - T_final.  Returns (color [F,3,H,W], radii [F,P], depth [F,1,H,W],
         alpha [F,1,H,W]); both maps are differentiable.  means2D_abs: see `forward`."""
-        if means2D_abs is not None:
-            return self._abs_grad(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
-                                  True, means2D_abs)
-        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
-        return _RasterizeGaussiansBatchDepthAlpha.apply(means3D, means2D, sh, col, opacities, sc, rot, cov,
-                                                        self.settings)
+        return tuple(self._maps(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                                depth_alpha=True, means2D_abs=means2D_abs).values())
 
     def forward_with_camera_grad(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None,
                                  rotations=None, cov3D_precomp=None, depth_alpha=False, means2D_abs=None):
@@ -1180,23 +912,8 @@ class BatchGaussianRasterizer(nn.Module):
         frame's settings.viewmatrix, settings.projmatrix and settings.campos: gradients reach those tensors that
         require them (stacked with autograd).  Intrinsics (tanfovx / tanfovy) are not differentiated.
         means2D_abs: see `forward`."""
-        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
-        views = torch.stack([s.viewmatrix for s in self.settings])
-        projs = torch.stack([s.projmatrix for s in self.settings])
-        campos = torch.stack([s.campos for s in self.settings])
-        return _RasterizeGaussiansBatchCam.apply(means3D, means2D, sh, col, opacities, sc, rot, cov, views, projs,
-                                                 campos, self.settings, bool(depth_alpha), means2D_abs)
-
-    def _abs_grad(self, means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
-                  depth_alpha, means2D_abs):
-        """`forward` / `forward_depth_alpha` with means2D_abs: the camera-input Function, cameras not differentiated."""
-        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
-        views = torch.stack([s.viewmatrix.detach() for s in self.settings])
-        projs = torch.stack([s.projmatrix.detach() for s in self.settings])
-        campos = torch.stack([s.campos.detach() for s in self.settings])
-        return _RasterizeGaussiansBatchCam.apply(means3D, means2D, sh, col, opacities, sc, rot, cov, views, projs,
-                                                 campos, self.settings, depth_alpha, means2D_abs)
-
+        return tuple(self._maps(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                                depth_alpha=depth_alpha, camera_grad=True, means2D_abs=means2D_abs).values())
 
     def forward_normal(self, means3D, means2D, opacities, normals, shs=None, colors_precomp=None, scales=None,
                        rotations=None, cov3D_precomp=None, camera_grad=False, means2D_abs=None):
@@ -1205,14 +922,10 @@ class BatchGaussianRasterizer(nn.Module):
         given (see GaussianRasterizer.forward_normal).  camera_grad=True: also differentiable with respect to each
         frame's settings.viewmatrix, .projmatrix and .campos (see `forward_with_camera_grad`).  means2D_abs: see
         `forward`.  Returns (color [F,3,H,W], radii [F,P], depth [F,1,H,W], alpha [F,1,H,W], normal [F,3,H,W])."""
-        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
-        views = projs = campos = None
-        if camera_grad:
-            views = torch.stack([s.viewmatrix for s in self.settings])
-            projs = torch.stack([s.projmatrix for s in self.settings])
-            campos = torch.stack([s.campos for s in self.settings])
-        return _RasterizeGaussiansBatchNormal.apply(means3D, means2D, sh, col, opacities, sc, rot, cov, normals, views,
-                                                    projs, campos, self.settings, means2D_abs)
+        if normals is None:
+            raise ValueError("normals must have dimensions (num_points, 3) or (num_frames, num_points, 3)")
+        return tuple(self._maps(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                                normals=normals, camera_grad=camera_grad, means2D_abs=means2D_abs).values())
 
     def forward_surface(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None,
                         rotations=None, cov3D_precomp=None, normals=None, near=0.2, far=100.0, camera_grad=False,
@@ -1221,16 +934,9 @@ class BatchGaussianRasterizer(nn.Module):
         GaussianRasterizer.forward_surface); with `normals` ([P,3] shared or [F,P,3] per frame) also the normal maps
         of `forward_normal`.  means2D_abs: see `forward`.  Returns (color [F,3,H,W], radii [F,P], depth, alpha,
         median_depth, distortion [F,1,H,W] each[, normal [F,3,H,W]]); every map is differentiable."""
-        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
-        views = projs = campos = None
-        if camera_grad:
-            views = torch.stack([s.viewmatrix for s in self.settings])
-            projs = torch.stack([s.projmatrix for s in self.settings])
-            campos = torch.stack([s.campos for s in self.settings])
-        return _RasterizeGaussiansBatchSurface.apply(means3D, means2D, sh, col, opacities, sc, rot, cov, normals,
-                                                     views, projs, campos, self.settings, float(near), float(far),
-                                                     means2D_abs)
-
+        return tuple(self._maps(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                                normals=normals, surface=(near, far), camera_grad=camera_grad,
+                                means2D_abs=means2D_abs).values())
 
     def forward_features(self, means3D, means2D, opacities, features, shs=None, colors_precomp=None, scales=None,
                          rotations=None, cov3D_precomp=None, camera_grad=False, normals=None, surface=None):
@@ -1241,15 +947,15 @@ class BatchGaussianRasterizer(nn.Module):
         `forward_normal`, with `surface` = (near, far) also the maps of `forward_surface`.  Returns (color
         [F,3,H,W], radii [F,P], depth [F,1,H,W], alpha [F,1,H,W], features [F,C,H,W][, median_depth, distortion
         [F,1,H,W]][, normal [F,3,H,W]]); every map is differentiable."""
-        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
-        views = projs = campos = None
-        if camera_grad:
-            views = torch.stack([s.viewmatrix for s in self.settings])
-            projs = torch.stack([s.projmatrix for s in self.settings])
-            campos = torch.stack([s.campos for s in self.settings])
-        surface = None if surface is None else (float(surface[0]), float(surface[1]))
-        return _RasterizeGaussiansBatchFeatures.apply(means3D, means2D, sh, col, opacities, sc, rot, cov, features,
-                                                      normals, views, projs, campos, self.settings, surface)
+        if features is None:
+            raise ValueError(f"features must have dimensions (num_points, C) or (num_frames, num_points, C), "
+                             f"1 <= C <= {_MAX_FEATURES}")
+        m = self._maps(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                       normals=normals, surface=surface, features=features, camera_grad=camera_grad)
+        f = m.pop("features")
+        out = tuple(m.values())
+        return out[:4] + (f,) + out[4:]
+
 
 class GaussianRasterizationSettings(NamedTuple):
     image_height: int
@@ -1299,14 +1005,26 @@ class GaussianRasterizer(nn.Module):
         return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
                                    raster_settings)
 
+    def _maps(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
+              cov3D_precomp=None, depth_alpha=False, normals=None, surface=None, features=None, camera_grad=False,
+              means2D_abs=None):
+        """The outputs by name, in _MAPS order: "color" and "radii"; "depth" and "alpha" with depth_alpha or any
+        other map; "median_depth" and "distortion" with surface = (near, far); "normal" with normals [P,3];
+        "features" with features [P,C].  camera_grad: see `forward_with_camera_grad`.  means2D_abs: see
+        `forward_abs_grad` (not with features)."""
+        rs = self.raster_settings
+        cams = (rs.viewmatrix, rs.projmatrix, rs.campos) if camera_grad else (None, None, None)
+        return _request_maps(_RasterizeGaussians, _RasterizeGaussiansMaps, rs, cams, means3D, means2D, opacities, shs,
+                             colors_precomp, scales, rotations, cov3D_precomp, depth_alpha, normals, surface,
+                             features, means2D_abs)
+
     def forward_depth_alpha(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None,
                             rotations=None, cov3D_precomp=None):
         """`forward` + the depth map sum_i d_i alpha_i T_i (view-space depth, unnormalised: expected depth is
         depth / alpha) and the alpha map 1 - T_final, over the same blend as the colour image.  Returns
         (color [3,H,W], radii [P], depth [1,H,W], alpha [1,H,W]); both maps are differentiable."""
-        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
-        return _RasterizeGaussiansDepthAlpha.apply(means3D, means2D, sh, col, opacities, sc, rot, cov,
-                                                   self.raster_settings)
+        return tuple(self._maps(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                                depth_alpha=True).values())
 
     def forward_with_camera_grad(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None,
                                  rotations=None, cov3D_precomp=None, depth_alpha=False):
@@ -1314,10 +1032,8 @@ class GaussianRasterizer(nn.Module):
         raster_settings.viewmatrix, .projmatrix and .campos: gradients reach those of the three tensors that require
         them, e.g. for a learnable pose correction (gaussian_renderer.posed_camera).  Intrinsics (tanfovx /
         tanfovy) are not differentiated.  Returns what `forward` / `forward_depth_alpha` return."""
-        rs = self.raster_settings
-        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
-        return _RasterizeGaussiansCam.apply(means3D, means2D, sh, col, opacities, sc, rot, cov, rs.viewmatrix,
-                                            rs.projmatrix, rs.campos, rs, bool(depth_alpha))
+        return tuple(self._maps(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                                depth_alpha=depth_alpha, camera_grad=True).values())
 
     def forward_abs_grad(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None,
                          rotations=None, cov3D_precomp=None, *, means2D_abs, depth_alpha=False, camera_grad=False):
@@ -1328,14 +1044,8 @@ class GaussianRasterizer(nn.Module):
         over every loss on the returned maps.  Unlike dL/dmean2D it does not cancel where pixels pull a Gaussian in
         opposite directions, which makes it a densification statistic that also splits large Gaussians over fine
         detail.  Returns what `forward` / `forward_depth_alpha` return."""
-        rs = self.raster_settings
-        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
-        view, proj, campos = rs.viewmatrix, rs.projmatrix, rs.campos
-        if not camera_grad:
-            view, proj, campos = view.detach(), proj.detach(), campos.detach()
-        return _RasterizeGaussiansCam.apply(means3D, means2D, sh, col, opacities, sc, rot, cov, view, proj, campos, rs,
-                                            bool(depth_alpha), means2D_abs)
-
+        return tuple(self._maps(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                                depth_alpha=depth_alpha, camera_grad=camera_grad, means2D_abs=means2D_abs).values())
 
     def forward_normal(self, means3D, means2D, opacities, normals, shs=None, colors_precomp=None, scales=None,
                        rotations=None, cov3D_precomp=None, camera_grad=False, means2D_abs=None):
@@ -1346,13 +1056,10 @@ class GaussianRasterizer(nn.Module):
         respect to raster_settings.viewmatrix, .projmatrix and .campos (see `forward_with_camera_grad`).  Returns
         (color [3,H,W], radii [P], depth [1,H,W], alpha [1,H,W], normal [3,H,W]); every map is differentiable.
         means2D_abs: see `forward_abs_grad`."""
-        rs = self.raster_settings
-        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
-        view, proj, campos = rs.viewmatrix, rs.projmatrix, rs.campos
-        if not camera_grad:
-            view, proj, campos = view.detach(), proj.detach(), campos.detach()
-        return _RasterizeGaussiansNormal.apply(means3D, means2D, sh, col, opacities, sc, rot, cov, normals, view, proj,
-                                               campos, rs, means2D_abs)
+        if normals is None:
+            raise ValueError("normals must have dimensions (num_points, 3)")
+        return tuple(self._maps(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                                normals=normals, camera_grad=camera_grad, means2D_abs=means2D_abs).values())
 
     def forward_surface(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None,
                         rotations=None, cov3D_precomp=None, normals=None, near=0.2, far=100.0, camera_grad=False,
@@ -1367,14 +1074,9 @@ class GaussianRasterizer(nn.Module):
         respect to raster_settings.viewmatrix, .projmatrix and .campos.  Returns (color [3,H,W], radii [P], depth,
         alpha, median_depth, distortion [1,H,W] each[, normal [3,H,W]]); every map is differentiable.  means2D_abs: see
         `forward_abs_grad`."""
-        rs = self.raster_settings
-        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
-        view, proj, campos = rs.viewmatrix, rs.projmatrix, rs.campos
-        if not camera_grad:
-            view, proj, campos = view.detach(), proj.detach(), campos.detach()
-        return _RasterizeGaussiansSurface.apply(means3D, means2D, sh, col, opacities, sc, rot, cov, normals, view,
-                                                proj, campos, rs, float(near), float(far), means2D_abs)
-
+        return tuple(self._maps(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                                normals=normals, surface=(near, far), camera_grad=camera_grad,
+                                means2D_abs=means2D_abs).values())
 
     def forward_features(self, means3D, means2D, opacities, features, shs=None, colors_precomp=None, scales=None,
                          rotations=None, cov3D_precomp=None, camera_grad=False):
@@ -1384,13 +1086,11 @@ class GaussianRasterizer(nn.Module):
         canonical coordinates for dense correspondences.  camera_grad=True: also differentiable with respect to
         raster_settings.viewmatrix, .projmatrix and .campos.  Returns (color [3,H,W], radii [P], depth [1,H,W], alpha
         [1,H,W], features [C,H,W]); every map is differentiable."""
-        rs = self.raster_settings
-        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
-        view, proj, campos = rs.viewmatrix, rs.projmatrix, rs.campos
-        if not camera_grad:
-            view, proj, campos = view.detach(), proj.detach(), campos.detach()
-        return _RasterizeGaussiansFeatures.apply(means3D, means2D, sh, col, opacities, sc, rot, cov, features, view,
-                                                 proj, campos, rs)
+        if features is None:
+            raise ValueError(f"features must have dimensions (num_points, C), 1 <= C <= {_MAX_FEATURES}")
+        return tuple(self._maps(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
+                                features=features, camera_grad=camera_grad).values())
+
 
 class _CCompat:
     """`diff_gaussian_rasterization._C` with the reference's three entry points and tuple

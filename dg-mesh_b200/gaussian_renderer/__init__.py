@@ -189,11 +189,10 @@ def render_flow(viewpoint_camera, cam_to, pc, pipe, bg_color, d_xyz, d_rotation,
     (FLOW_NEAR, the rasterizer's near cut-off) contributes zero flow and receives no flow gradient.  Supervise
     flow / alpha (or flow against alpha times an estimate) with an off-line optical-flow estimate.  abs_grad=True
     raises ValueError, as for `render_features`."""
-    _refuse_abs_grad(abs_grad)
     x = pc.get_xyz
     f = flow_features(viewpoint_camera, cam_to, x + d_xyz, x + d_xyz_to)
     out = _render(viewpoint_camera, pc, pipe, bg_color, d_xyz, d_rotation, d_scaling, False, scaling_modifier,
-                  override_color, True, camera_grad=camera_grad, features=f)
+                  override_color, True, camera_grad=camera_grad, features=f, abs_grad=abs_grad)
     out["flow"] = out.pop("features")
     return out
 
@@ -256,12 +255,6 @@ def _se3_exp(delta):
     return rp_to_se3(R[None], (V @ v)[None, :, None])[0]
 
 
-def _refuse_abs_grad(abs_grad):
-    # the feature pass adds its dL/dalpha in a pass of its own, so no per-pixel total exists to take |.| of
-    if abs_grad:
-        raise ValueError("abs_grad: the absolute screen-space gradient is not available with feature or flow maps")
-
-
 def _viewspace_points(shape, dtype):
     """Zero tensor whose gradient receives a screen-space statistic of the 2D means (densification)."""
     t = torch.zeros(shape, dtype=dtype, requires_grad=True, device="cuda") + 0
@@ -274,8 +267,6 @@ def _viewspace_points(shape, dtype):
 
 def _render(viewpoint_camera, pc, pipe, bg_color, d_xyz, d_rotation, d_scaling, is_6dof, scaling_modifier,
             override_color, depth_alpha, camera_grad=False, normals=None, surface=None, features=None, abs_grad=False):
-    if features is not None:
-        _refuse_abs_grad(abs_grad)
     # zero tensor whose gradient receives the 2D (screen-space) mean gradients (densification statistics)
     screenspace_points = torch.zeros_like(pc.get_xyz, dtype=pc.get_xyz.dtype, requires_grad=True,
                                           device="cuda") + 0
@@ -287,44 +278,17 @@ def _render(viewpoint_camera, pc, pipe, bg_color, d_xyz, d_rotation, d_scaling, 
     kw = _gaussian_inputs(viewpoint_camera, pc, pipe, d_xyz, d_rotation, d_scaling, is_6dof, scaling_modifier,
                           override_color)
     points_abs = _viewspace_points(pc.get_xyz.shape, pc.get_xyz.dtype) if abs_grad else None
-    if points_abs is not None:
-        kw["means2D_abs"] = points_abs
-    if features is not None:
-        out = rasterizer.forward_features(means2D=screenspace_points, features=features, camera_grad=camera_grad, **kw)
-    elif surface is not None:
-        out = rasterizer.forward_surface(means2D=screenspace_points, normals=normals, near=surface[0], far=surface[1],
-                                         camera_grad=camera_grad, **kw)
-    elif normals is not None:
-        out = rasterizer.forward_normal(means2D=screenspace_points, normals=normals, camera_grad=camera_grad, **kw)
-    elif points_abs is not None:
-        out = rasterizer.forward_abs_grad(means2D=screenspace_points, depth_alpha=depth_alpha, camera_grad=camera_grad,
-                                          **kw)
-    elif camera_grad:
-        out = rasterizer.forward_with_camera_grad(means2D=screenspace_points, depth_alpha=depth_alpha, **kw)
-    elif depth_alpha:
-        out = rasterizer.forward_depth_alpha(means2D=screenspace_points, **kw)
-    else:
-        out = rasterizer(means2D=screenspace_points, **kw)
-    if not depth_alpha:
-        rendered_image, radii = out
-        res = {"render": rendered_image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0,
-               "radii": radii}
-        if points_abs is not None:
-            res["viewspace_points_abs"] = points_abs
-        return res
-    rendered_image, radii, depth, alpha = out[:4]
-    res = {"render": rendered_image, "viewspace_points": screenspace_points, "visibility_filter": radii > 0,
-           "radii": radii, "depth": depth, "alpha": alpha}
+    maps = rasterizer._maps(means2D=screenspace_points, depth_alpha=depth_alpha, camera_grad=camera_grad,
+                            normals=normals, surface=surface, features=features, means2D_abs=points_abs, **kw)
+    return _result(maps, screenspace_points, points_abs)
+
+
+def _result(maps, screenspace_points, points_abs):
+    """The result dict of `render` / `render_batch` from the rasterizer's maps by name."""
+    res = {"render": maps.pop("color"), "viewspace_points": screenspace_points, "visibility_filter": maps["radii"] > 0}
+    res.update(maps)
     if points_abs is not None:
         res["viewspace_points_abs"] = points_abs
-    if features is not None:
-        res["features"] = out[4]
-    elif surface is not None:
-        res["median_depth"], res["distortion"] = out[4], out[5]
-        if normals is not None:
-            res["normal"] = out[6]
-    elif normals is not None:
-        res["normal"] = out[4]
     return res
 
 
@@ -350,8 +314,6 @@ def render_batch(cameras, pc, pipe, bg_color, d_xyz, d_rotation, d_scaling, scal
     with each other (one pass over C + 2 channels) and with the other maps; they add "depth" and "alpha".
     abs_grad=True adds "viewspace_points_abs" [F,N,3] (see `render_abs_grad`), each frame's statistic in its slab;
     not with features or flow_to (ValueError)."""
-    if features is not None or flow_to is not None:
-        _refuse_abs_grad(abs_grad)
     F, N = len(cameras), pc.get_xyz.shape[0]
     screenspace_points = torch.zeros((F, N, 3), dtype=pc.get_xyz.dtype, requires_grad=True, device="cuda") + 0
     try:
@@ -377,49 +339,16 @@ def render_batch(cameras, pc, pipe, bg_color, d_xyz, d_rotation, d_scaling, scal
               rotations=pc.get_rotation + d_rotation, shs=pc.get_features)
     rasterizer = BatchGaussianRasterizer(sets)
     points_abs = _viewspace_points((F, N, 3), pc.get_xyz.dtype) if abs_grad else None
-    if points_abs is not None:
-        kw["means2D_abs"] = points_abs
     feats, C = _batch_features(cameras, pc, F, d_xyz, features, flow_to, per_frame)
+    maps = rasterizer._maps(means2D=screenspace_points, depth_alpha=depth_alpha, camera_grad=camera_grad, normals=nrm,
+                            surface=(near, far) if surface else None, features=feats, means2D_abs=points_abs, **kw)
     if feats is not None:
-        out = rasterizer.forward_features(means2D=screenspace_points, features=feats, camera_grad=camera_grad,
-                                          normals=nrm, surface=(near, far) if surface else None, **kw)
-        out = out[:4] + out[5:] + (out[4],)
-    elif surface:
-        out = rasterizer.forward_surface(means2D=screenspace_points, normals=nrm, near=near, far=far,
-                                         camera_grad=camera_grad, **kw)
-    elif nrm is not None:
-        out = rasterizer.forward_normal(means2D=screenspace_points, normals=nrm, camera_grad=camera_grad, **kw)
-    elif camera_grad:
-        out = rasterizer.forward_with_camera_grad(means2D=screenspace_points, depth_alpha=depth_alpha, **kw)
-    elif depth_alpha:
-        out = rasterizer.forward_depth_alpha(means2D=screenspace_points, **kw)
-    else:
-        out = rasterizer(means2D=screenspace_points, **kw)
-    if not (depth_alpha or normals or surface or feats is not None):
-        images, radii = out
-        res = {"render": images, "viewspace_points": screenspace_points, "visibility_filter": radii > 0,
-               "radii": radii}
-        if points_abs is not None:
-            res["viewspace_points_abs"] = points_abs
-        return res
-    images, radii, depth, alpha = out[:4]
-    res = {"render": images, "viewspace_points": screenspace_points, "visibility_filter": radii > 0, "radii": radii,
-           "depth": depth, "alpha": alpha}
-    if points_abs is not None:
-        res["viewspace_points_abs"] = points_abs
-    if surface:
-        res["median_depth"], res["distortion"] = out[4], out[5]
-        if nrm is not None:
-            res["normal"] = out[6]
-    elif nrm is not None:
-        res["normal"] = out[4]
-    if feats is not None:
-        fm = out[-1]
+        fm = maps.pop("features")
         if features is not None:
-            res["features"] = fm[:, :C]
+            maps["features"] = fm[:, :C]
         if flow_to is not None:
-            res["flow"] = fm[:, C:]
-    return res
+            maps["flow"] = fm[:, C:]
+    return _result(maps, screenspace_points, points_abs)
 
 
 def _batch_features(cameras, pc, F, d_xyz, features, flow_to, per_frame):
