@@ -185,7 +185,7 @@ __global__ void __launch_bounds__(256) dpsr_finalize_kernel(size_t n, int N, flo
 // ================================================================== backward
 // 1. g = dL/dout -> dphi (grid), with the contributions through fv0 and through the mean shift.
 //    out = k * phi1 with k = -0.5/|fv0| (mode 0) or 0.5/fv0 (mode 1); phi1 = phi - offset.
-//    Two-pass: (a) reduce A = sum g_i, B = sum g_i phi1_i ; (b) write dphi.
+//    Two-pass: (a) reduce A = sum g_i, B = sum g_i phi1_i over i >= 1 ; (b) write dphi.
 __global__ void __launch_bounds__(256) dpsr_bwd_reduce_kernel(size_t n, float inv_n3, const float* __restrict__ g,
                                                               const float* __restrict__ phi_raw,
                                                               const float* __restrict__ scal,
@@ -193,6 +193,7 @@ __global__ void __launch_bounds__(256) dpsr_bwd_reduce_kernel(size_t n, float in
   const float offset = scal[0];
   double a = 0, b = 0;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    if (i == 0) continue;  // out_0 is constant: see dpsr_bwd_dphi_kernel
     const float gi = g[i];
     a += gi;
     b += (double)gi * (double)(phi_raw[i] * inv_n3 - offset);
@@ -216,8 +217,11 @@ __global__ void __launch_bounds__(256) dpsr_bwd_reduce_kernel(size_t n, float in
   }
 }
 
-// dphi_i = k g_i (+ dfv0 at i = 0); doffset = -(sum_i dphi_i); dthres = -sum g (mode 1).
+// dphi_i = k g_i for i >= 1, dphi_0 = dfv0; doffset = -(sum_i dphi_i); dthres = -sum g (mode 1).
 // coef[0] = doffset / N  (the gradient every point's interpolated value receives).
+// out_0 = k * fv0 is constant (-0.5 sign(fv0), or 0.5 - thres), so g_0 reaches nothing but thres: its direct term
+// k g_0 and its term through fv0, dk g_0 fv0, cancel exactly.  Both are left out (A and B skip i = 0) instead of
+// leaving the rounding of that cancellation in every gradient.
 __global__ void __launch_bounds__(256) dpsr_bwd_dphi_kernel(size_t n, int N, const float* __restrict__ g,
                                                             const float* __restrict__ scal,
                                                             const double* __restrict__ red, int mode,
@@ -232,10 +236,10 @@ __global__ void __launch_bounds__(256) dpsr_bwd_dphi_kernel(size_t n, int N, con
   if (i == 0) {
     const double sum_dphi = (double)k * red[0] + (double)dfv0;
     coef[0] = (float)(-sum_dphi / (double)N);
-    if (dthres) dthres[0] = mode ? (float)(-red[0]) : 0.f;
+    if (dthres) dthres[0] = mode ? (float)(-(red[0] + (double)g[0])) : 0.f;
   }
   if (i >= n) return;
-  dphi[i] = k * g[i] + (i == 0 ? dfv0 : 0.f);
+  dphi[i] = i == 0 ? dfv0 : k * g[i];
 }
 
 // 2. every point's interpolated value fv_p gets the same gradient c = doffset/N:
