@@ -154,85 +154,169 @@ int normal_args(int P, int64_t R_cap, const float* normals, float* out_normal, v
   return DGM_OK;
 }
 
-int forward_one(int P, int D, int M, const float* background, int W, int H, const float* means3D, const float* shs,
-                const float* colors_precomp, const float* opacities, const float* scales, float scale_modifier,
-                const float* rotations, const float* cov3D_precomp, const float* viewmatrix, const float* projmatrix,
-                const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered, float* out_color, int* radii,
-                float* out_depth, float* out_alpha, const float* normals, float* out_normal, void* nrm_ws,
-                size_t nrm_ws_bytes, float near_, float far_, float* out_median, float* out_distortion,
-                void* surf_ws, size_t surf_ws_bytes, void* geom_ws, size_t geom_bytes, void* binning_ws,
-                size_t binning_bytes,
-                int64_t R_cap, void* img_ws, size_t img_bytes, int32_t* status, int32_t* status_host,
-                void* status_event, float depth_hint_lo, float depth_hint_hi, int max_tile_hint, void* stream) {
-  if (P < 0 || W <= 0 || H <= 0 || R_cap < 0) return bad("dgr_forward: negative size");
-  if (!background || !viewmatrix || !projmatrix || !cam_pos || !out_color || !status)
-    return bad("dgr_forward: null required pointer");
-  int rc = normal_args(P, R_cap, normals, out_normal, nrm_ws, nrm_ws_bytes);
-  if (rc != DGM_OK) return rc;
+// the Gaussian inputs of a forward of P > 0 Gaussians: DGM_OK, or the error to return (`who` names the entry point)
+int gaussian_args(const char* who, int D, int M, const float* means3D, const float* shs, const float* colors_precomp,
+                  const float* opacities, const float* scales, const float* rotations, const float* cov3D_precomp) {
+  const char* e = nullptr;
+  if (!means3D || !opacities) e = "means3D / opacities missing";
+  else if ((shs == nullptr) == (colors_precomp == nullptr)) e = "exactly one of shs / colors_precomp";
+  else if (((scales == nullptr) || (rotations == nullptr)) == (cov3D_precomp == nullptr))
+    e = "exactly one of scales+rotations / cov3D_precomp";
+  else if (shs && (M <= 0 || M > 16 || (D + 1) * (D + 1) > M || D < 0 || D > 3)) e = "SH degree / coefficient count";
+  if (!e) return DGM_OK;
+  char msg[128];
+  snprintf(msg, sizeof(msg), "%s: %s", who, e);
+  return bad(msg);
+}
+
+// Internal streams for the frame batches (created once per process).
+//   hi[]  high priority: the short, latency-bound kernels (preprocess / binning / sort)
+//   lo[]  low priority : the blend kernels, each of which fills the GPU on its own; two streams,
+//         alternating frames, so the next kernel's CTAs fill the SMs while the previous one's tail drains
+// A frame's binning chain runs on hi[f % NH] and its blend kernel on lo behind an event.  The block
+// scheduler serves pending high-priority CTAs first, so the binning chains of the NEXT frames slip
+// through while the blend kernel of the current frame is running (they are latency-bound and cost
+// the issue-bound blend kernel almost nothing) instead of queueing behind its 2 500 CTAs.
+struct BatchStreams {
+  static const int NH = 4;
+  cudaStream_t hi[NH] = {}, lo[2] = {};
+  cudaEvent_t fork = nullptr, done_hi[NH] = {}, done_lo[2] = {}, ready[NH] = {};
+  bool ok = false;
+  std::mutex mu;  // one batch call at a time per device (the events above are shared)
+  bool init() {
+    if (ok) return true;
+    int least = 0, greatest = 0;
+    if (cudaDeviceGetStreamPriorityRange(&least, &greatest) != cudaSuccess) return false;
+    for (int i = 0; i < NH; ++i) {
+      if (cudaStreamCreateWithPriority(&hi[i], cudaStreamNonBlocking, greatest) != cudaSuccess) return false;
+      if (cudaEventCreateWithFlags(&done_hi[i], cudaEventDisableTiming) != cudaSuccess) return false;
+      if (cudaEventCreateWithFlags(&ready[i], cudaEventDisableTiming) != cudaSuccess) return false;
+    }
+    if (cudaEventCreateWithFlags(&fork, cudaEventDisableTiming) != cudaSuccess) return false;
+    for (int i = 0; i < 2; ++i) {
+      if (cudaStreamCreateWithPriority(&lo[i], cudaStreamNonBlocking, least) != cudaSuccess) return false;
+      if (cudaEventCreateWithFlags(&done_lo[i], cudaEventDisableTiming) != cudaSuccess) return false;
+    }
+    ok = true;
+    return true;
+  }
+};
+// one set per device, created on first use
+std::mutex g_bs_mu;
+std::map<int, BatchStreams*> g_bs_map;
+BatchStreams* batch_streams() {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
+  std::lock_guard<std::mutex> lk(g_bs_mu);
+  BatchStreams*& p = g_bs_map[dev];
+  if (!p) p = new BatchStreams();
+  return p->init() ? p : nullptr;
+}
+
+// a frame of no Gaussian: the reference skips the whole pipeline and returns the zero-initialised image
+// (rasterize_points.cu:64,80: torch::full(0.0) and `if (P != 0)`)
+cudaError_t zero_frame(const dgm::FwdArgs& a, cudaStream_t s) {
+  const size_t map = sizeof(float) * (size_t)a.W * a.H;
+  cudaMemsetAsync(a.out_color, 0, 3 * map, s);
+  if (a.out_depth) cudaMemsetAsync(a.out_depth, 0, map, s);
+  if (a.out_alpha) cudaMemsetAsync(a.out_alpha, 0, map, s);
+  if (a.out_normal) cudaMemsetAsync(a.out_normal, 0, 3 * map, s);
+  if (a.out_median) cudaMemsetAsync(a.out_median, 0, map, s);
+  if (a.out_distortion) cudaMemsetAsync(a.out_distortion, 0, map, s);
+  cudaMemsetAsync(a.status, 0, sizeof(int32_t) * DGR_STATUS_WORDS, s);
+  if (a.status_host) memset(a.status_host, 0, sizeof(int32_t) * DGR_STATUS_WORDS);
+  if (a.status_event) cudaEventRecord(a.status_event, s);
+  return cudaGetLastError();
+}
+
+// The forward of F frames whose arguments have been checked, in the layout of dgr_forward_batch_surf (one frame: the
+// arguments of dgr_forward_surf with F = 1, strides 0 and one stream).  Frame f reads camera f and the slab f of each
+// per-frame input, and writes its maps, radii and status words at f times their size and its workspaces at f times
+// their stride.  With one stream (or one frame, or no Gaussian) the frames run in order on the caller's stream and
+// status_event is recorded after the last frame's tile scan; otherwise they run on the BatchStreams.
+int forward_frames(int F, int P, int D, int M, const float* background, int W, int H, const float* means3D,
+                   const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
+                   float scale_modifier, const float* rotations, const float* cov3D_precomp, int per_frame,
+                   const float* viewmatrices, const float* projmatrices, const float* cam_poses,
+                   const float* tan_fovx_host, const float* tan_fovy_host, int prefiltered, float* out_color,
+                   int* radii, float* out_depth, float* out_alpha, const float* normals, int normals_per_frame,
+                   float* out_normal, void* nrm_ws, size_t nrm_ws_stride, float near_, float far_,
+                   float* out_median, float* out_distortion, void* surf_ws, size_t surf_ws_stride, void* geom_ws,
+                   size_t geom_stride, void* binning_ws, size_t binning_stride, int64_t R_cap, void* img_ws,
+                   size_t img_stride, int32_t* status, int32_t* status_host, void* status_event,
+                   float depth_hint_lo, float depth_hint_hi, int max_tile_hint, int n_streams, void* stream) {
+  const size_t npix = (size_t)W * H, cw = shs ? (size_t)M * 3 : 3;
   const bool surf = out_median || out_distortion;
-  if (surf && (rc = surface_args(W, H, near_, far_, surf_ws, surf_ws_bytes)) != DGM_OK) return rc;
-  if (P > 0) {
-    if (!means3D || !opacities) return bad("dgr_forward: means3D / opacities missing");
-    if ((shs == nullptr) == (colors_precomp == nullptr)) return bad("dgr_forward: exactly one of shs / colors_precomp");
-    if (((scales == nullptr) || (rotations == nullptr)) == (cov3D_precomp == nullptr))
-      return bad("dgr_forward: exactly one of scales+rotations / cov3D_precomp");
-    if (shs && (M <= 0 || M > 16 || (D + 1) * (D + 1) > M || D < 0 || D > 3))
-      return bad("dgr_forward: SH degree / coefficient count");
+  // frame f of: an input whose bit is set in per_frame ([F,P,width]), a [F,c,H,W] map, a workspace
+  auto pf = [&](const float* p, int bit, size_t width, int f) {
+    return (p && (per_frame & bit)) ? p + (size_t)f * P * width : p;
+  };
+  auto map = [&](float* p, size_t c, int f) { return p ? p + f * c * npix : p; };
+  auto ws = [](void* p, size_t stride, int f) { return p ? (void*)((char*)p + f * stride) : p; };
+  auto frame = [&](int f) {
+    dgm::FwdArgs a;
+    a.P = P; a.D = D; a.M = M; a.background = background; a.W = W; a.H = H;
+    a.means3D = pf(means3D, DGR_PF_MEANS, 3, f); a.shs = pf(shs, DGR_PF_COLOR, cw, f);
+    a.colors_precomp = pf(colors_precomp, DGR_PF_COLOR, 3, f); a.opacities = pf(opacities, DGR_PF_OPAC, 1, f);
+    a.scales = pf(scales, DGR_PF_SCALES, 3, f); a.scale_modifier = scale_modifier;
+    a.rotations = pf(rotations, DGR_PF_ROTS, 4, f); a.cov3D_precomp = pf(cov3D_precomp, DGR_PF_COV, 6, f);
+    a.viewmatrix = viewmatrices + 16 * f; a.projmatrix = projmatrices + 16 * f; a.cam_pos = cam_poses + 3 * f;
+    a.tan_fovx = tan_fovx_host[f]; a.tan_fovy = tan_fovy_host[f]; a.prefiltered = prefiltered;
+    a.out_color = map(out_color, 3, f); a.radii = radii ? radii + (size_t)f * P : nullptr;
+    a.out_depth = map(out_depth, 1, f); a.out_alpha = map(out_alpha, 1, f);
+    a.geom_ws = ws(geom_ws, geom_stride, f); a.binning_ws = ws(binning_ws, binning_stride, f);
+    a.img_ws = ws(img_ws, img_stride, f); a.R_cap = R_cap;
+    a.status = status + f * DGR_STATUS_WORDS; a.status_host = status_host ? status_host + f * DGR_STATUS_WORDS : nullptr;
+    a.status_event = nullptr; a.hint_lo = depth_hint_lo; a.hint_hi = depth_hint_hi; a.hint_max_tile = max_tile_hint;
+    if (out_normal) {
+      a.normals = (normals && normals_per_frame) ? normals + (size_t)f * P * 3 : normals;
+      a.out_normal = map(out_normal, 3, f); a.nrm_ws = ws(nrm_ws, nrm_ws_stride, f);
+    }
+    if (surf) {
+      a.out_median = map(out_median, 1, f); a.out_distortion = map(out_distortion, 1, f);
+      a.surf_ws = ws(surf_ws, surf_ws_stride, f); a.surf_k = surf_k(near_, far_);
+    }
+    return a;
+  };
+  cudaStream_t main_s = (cudaStream_t)stream;
+  cudaError_t e = cudaSuccess;
+  if (n_streams <= 1 || F == 1 || P == 0) {
+    for (int f = 0; f < F && e == cudaSuccess; ++f) {
+      dgm::FwdArgs a = frame(f);
+      if (f == F - 1) a.status_event = (cudaEvent_t)status_event;
+      e = P > 0 ? dgm::launch_forward(a, main_s) : zero_frame(a, main_s);
+    }
+    return check(e);
   }
-  if (P == 0) {
-    // the reference skips the whole pipeline and returns the zero-initialised image
-    // (rasterize_points.cu:64,80: torch::full(0.0) and `if (P != 0)`)
-    cudaMemsetAsync(out_color, 0, sizeof(float) * 3 * (size_t)W * H, (cudaStream_t)stream);
-    if (out_depth) cudaMemsetAsync(out_depth, 0, sizeof(float) * (size_t)W * H, (cudaStream_t)stream);
-    if (out_alpha) cudaMemsetAsync(out_alpha, 0, sizeof(float) * (size_t)W * H, (cudaStream_t)stream);
-    if (out_normal) cudaMemsetAsync(out_normal, 0, sizeof(float) * 3 * (size_t)W * H, (cudaStream_t)stream);
-    if (out_median) cudaMemsetAsync(out_median, 0, sizeof(float) * (size_t)W * H, (cudaStream_t)stream);
-    if (out_distortion) cudaMemsetAsync(out_distortion, 0, sizeof(float) * (size_t)W * H, (cudaStream_t)stream);
-    cudaMemsetAsync(status, 0, sizeof(int32_t) * DGR_STATUS_WORDS, (cudaStream_t)stream);
-    if (status_host) memset(status_host, 0, sizeof(int32_t) * DGR_STATUS_WORDS);
-    if (status_event) cudaEventRecord((cudaEvent_t)status_event, (cudaStream_t)stream);
-    return check(cudaGetLastError());
+  const int NH = n_streams > BatchStreams::NH ? BatchStreams::NH : n_streams;
+  BatchStreams* bs = batch_streams();
+  if (!bs) return check(cudaGetLastError());
+  std::lock_guard<std::mutex> lk(bs->mu);
+  cudaEventRecord(bs->fork, main_s);
+  for (int i = 0; i < NH; ++i) cudaStreamWaitEvent(bs->hi[i], bs->fork, 0);
+  for (int i = 0; i < 2; ++i) cudaStreamWaitEvent(bs->lo[i], bs->fork, 0);
+  for (int f = 0; f < F && e == cudaSuccess; ++f) {
+    const int i = f % NH;
+    cudaStream_t lo = bs->lo[f & 1];
+    const dgm::FwdArgs a = frame(f);
+    e = dgm::launch_binning(a, bs->hi[i]);
+    cudaEventRecord(bs->ready[i], bs->hi[i]);
+    cudaStreamWaitEvent(lo, bs->ready[i], 0);
+    if (e == cudaSuccess) e = dgm::launch_render(a, lo);
   }
-  size_t gb, bb, ib;
-  dgr_workspace_sizes(P, W, H, R_cap, &gb, &bb, &ib);
-  if (geom_bytes < gb || binning_bytes < bb || img_bytes < ib || !geom_ws || !binning_ws || !img_ws) {
-    strncpy(g_last_error, "dgr_forward: workspace too small", sizeof(g_last_error) - 1);
-    return DGM_E_WORKSPACE;
+  // the binning chains finish long before the blend kernels: the caller's status event fires then
+  for (int i = 0; i < NH; ++i) {
+    cudaEventRecord(bs->done_hi[i], bs->hi[i]);
+    cudaStreamWaitEvent(main_s, bs->done_hi[i], 0);
   }
-  dgm::FwdArgs a;
-  a.P = P; a.D = D; a.M = M; a.background = background; a.W = W; a.H = H;
-  a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.opacities = opacities;
-  a.scales = scales; a.scale_modifier = scale_modifier; a.rotations = rotations; a.cov3D_precomp = cov3D_precomp;
-  a.viewmatrix = viewmatrix; a.projmatrix = projmatrix; a.cam_pos = cam_pos;
-  a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy; a.prefiltered = prefiltered;
-  a.out_color = out_color; a.radii = radii; a.out_depth = out_depth; a.out_alpha = out_alpha;
-  a.geom_ws = geom_ws; a.binning_ws = binning_ws; a.img_ws = img_ws; a.R_cap = R_cap; a.status = status;
-  a.status_host = status_host; a.status_event = (cudaEvent_t)status_event;
-  a.hint_lo = depth_hint_lo; a.hint_hi = depth_hint_hi; a.hint_max_tile = max_tile_hint;
-  if (out_normal) a.normals = normals, a.out_normal = out_normal, a.nrm_ws = nrm_ws;
-  if (surf) {
-    a.out_median = out_median; a.out_distortion = out_distortion; a.surf_ws = surf_ws;
-    a.surf_k = surf_k(near_, far_);
+  if (status_event) cudaEventRecord((cudaEvent_t)status_event, main_s);
+  for (int i = 0; i < 2; ++i) {
+    cudaEventRecord(bs->done_lo[i], bs->lo[i]);
+    cudaStreamWaitEvent(main_s, bs->done_lo[i], 0);
   }
-  return check(dgm::launch_forward(a, (cudaStream_t)stream));
+  return check(e != cudaSuccess ? e : cudaGetLastError());
 }
 }  // namespace
-
-int dgr_forward_aux(int P, int D, int M, const float* background, int W, int H, const float* means3D,
-                    const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
-                    float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
-                    const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered,
-                    float* out_color, int* radii, float* out_depth, float* out_alpha, void* geom_ws,
-                    size_t geom_bytes, void* binning_ws, size_t binning_bytes, int64_t R_cap, void* img_ws,
-                    size_t img_bytes, int32_t* status, int32_t* status_host, void* status_event,
-                    float depth_hint_lo, float depth_hint_hi, int max_tile_hint, void* stream) {
-  return forward_one(P, D, M, background, W, H, means3D, shs, colors_precomp, opacities, scales, scale_modifier,
-                     rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered,
-                     out_color, radii, out_depth, out_alpha, nullptr, nullptr, nullptr, 0, 0.f, 0.f, nullptr,
-                     nullptr, nullptr, 0, geom_ws, geom_bytes,
-                     binning_ws, binning_bytes, R_cap, img_ws, img_bytes, status, status_host, status_event,
-                     depth_hint_lo, depth_hint_hi, max_tile_hint, stream);
-}
 
 int dgr_forward_surf(int P, int D, int M, const float* background, int W, int H, const float* means3D,
                      const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
@@ -244,12 +328,28 @@ int dgr_forward_surf(int P, int D, int M, const float* background, int W, int H,
                      size_t geom_bytes, void* binning_ws, size_t binning_bytes, int64_t R_cap, void* img_ws,
                      size_t img_bytes, int32_t* status, int32_t* status_host, void* status_event,
                      float depth_hint_lo, float depth_hint_hi, int max_tile_hint, void* stream) {
-  return forward_one(P, D, M, background, W, H, means3D, shs, colors_precomp, opacities, scales, scale_modifier,
-                     rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered,
-                     out_color, radii, out_depth, out_alpha, normals, out_normal, nrm_ws, nrm_ws_bytes, near_, far_,
-                     out_median, out_distortion, surf_ws, surf_ws_bytes, geom_ws, geom_bytes, binning_ws,
-                     binning_bytes, R_cap, img_ws, img_bytes, status, status_host, status_event, depth_hint_lo,
-                     depth_hint_hi, max_tile_hint, stream);
+  if (P < 0 || W <= 0 || H <= 0 || R_cap < 0) return bad("dgr_forward: negative size");
+  if (!background || !viewmatrix || !projmatrix || !cam_pos || !out_color || !status)
+    return bad("dgr_forward: null required pointer");
+  int rc = normal_args(P, R_cap, normals, out_normal, nrm_ws, nrm_ws_bytes);
+  if (rc != DGM_OK) return rc;
+  if ((out_median || out_distortion) && (rc = surface_args(W, H, near_, far_, surf_ws, surf_ws_bytes)) != DGM_OK)
+    return rc;
+  if (P > 0) {
+    rc = gaussian_args("dgr_forward", D, M, means3D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp);
+    if (rc != DGM_OK) return rc;
+    size_t gb, bb, ib;
+    dgr_workspace_sizes(P, W, H, R_cap, &gb, &bb, &ib);
+    if (geom_bytes < gb || binning_bytes < bb || img_bytes < ib || !geom_ws || !binning_ws || !img_ws) {
+      strncpy(g_last_error, "dgr_forward: workspace too small", sizeof(g_last_error) - 1);
+      return DGM_E_WORKSPACE;
+    }
+  }
+  return forward_frames(1, P, D, M, background, W, H, means3D, shs, colors_precomp, opacities, scales, scale_modifier,
+                        rotations, cov3D_precomp, 0, viewmatrix, projmatrix, cam_pos, &tan_fovx, &tan_fovy,
+                        prefiltered, out_color, radii, out_depth, out_alpha, normals, 0, out_normal, nrm_ws, 0, near_,
+                        far_, out_median, out_distortion, surf_ws, 0, geom_ws, 0, binning_ws, 0, R_cap, img_ws, 0,
+                        status, status_host, status_event, depth_hint_lo, depth_hint_hi, max_tile_hint, 1, stream);
 }
 
 int dgr_forward_nrm(int P, int D, int M, const float* background, int W, int H, const float* means3D,
@@ -261,12 +361,28 @@ int dgr_forward_nrm(int P, int D, int M, const float* background, int W, int H, 
                     void* binning_ws, size_t binning_bytes, int64_t R_cap, void* img_ws, size_t img_bytes,
                     int32_t* status, int32_t* status_host, void* status_event, float depth_hint_lo,
                     float depth_hint_hi, int max_tile_hint, void* stream) {
-  return forward_one(P, D, M, background, W, H, means3D, shs, colors_precomp, opacities, scales, scale_modifier,
-                     rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered,
-                     out_color, radii, out_depth, out_alpha, normals, out_normal, nrm_ws, nrm_ws_bytes, 0.f, 0.f,
-                     nullptr, nullptr, nullptr, 0, geom_ws, geom_bytes, binning_ws, binning_bytes, R_cap, img_ws,
-                     img_bytes, status, status_host, status_event, depth_hint_lo, depth_hint_hi, max_tile_hint,
-                     stream);
+  return dgr_forward_surf(P, D, M, background, W, H, means3D, shs, colors_precomp, opacities, scales, scale_modifier,
+                          rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered,
+                          out_color, radii, out_depth, out_alpha, normals, out_normal, nrm_ws, nrm_ws_bytes, 0.f, 0.f,
+                          nullptr, nullptr, nullptr, 0, geom_ws, geom_bytes, binning_ws, binning_bytes, R_cap, img_ws,
+                          img_bytes, status, status_host, status_event, depth_hint_lo, depth_hint_hi, max_tile_hint,
+                          stream);
+}
+
+int dgr_forward_aux(int P, int D, int M, const float* background, int W, int H, const float* means3D,
+                    const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
+                    float scale_modifier, const float* rotations, const float* cov3D_precomp, const float* viewmatrix,
+                    const float* projmatrix, const float* cam_pos, float tan_fovx, float tan_fovy, int prefiltered,
+                    float* out_color, int* radii, float* out_depth, float* out_alpha, void* geom_ws,
+                    size_t geom_bytes, void* binning_ws, size_t binning_bytes, int64_t R_cap, void* img_ws,
+                    size_t img_bytes, int32_t* status, int32_t* status_host, void* status_event,
+                    float depth_hint_lo, float depth_hint_hi, int max_tile_hint, void* stream) {
+  return dgr_forward_surf(P, D, M, background, W, H, means3D, shs, colors_precomp, opacities, scales, scale_modifier,
+                          rotations, cov3D_precomp, viewmatrix, projmatrix, cam_pos, tan_fovx, tan_fovy, prefiltered,
+                          out_color, radii, out_depth, out_alpha, nullptr, nullptr, nullptr, 0, 0.f, 0.f, nullptr,
+                          nullptr, nullptr, 0, geom_ws, geom_bytes, binning_ws, binning_bytes, R_cap, img_ws,
+                          img_bytes, status, status_host, status_event, depth_hint_lo, depth_hint_hi, max_tile_hint,
+                          stream);
 }
 
 int dgr_forward(int P, int D, int M, const float* background, int W, int H, const float* means3D, const float* shs,
@@ -281,6 +397,108 @@ int dgr_forward(int P, int D, int M, const float* background, int W, int H, cons
                          out_color, radii, nullptr, nullptr, geom_ws, geom_bytes, binning_ws, binning_bytes, R_cap,
                          img_ws, img_bytes, status, status_host, status_event, depth_hint_lo, depth_hint_hi,
                          max_tile_hint, stream);
+}
+
+int dgr_forward_batch_surf(int F, int P, int D, int M, const float* background, int W, int H,
+                           const float* means3D, const float* shs, const float* colors_precomp,
+                           const float* opacities, const float* scales, float scale_modifier, const float* rotations,
+                           const float* cov3D_precomp, int per_frame, const float* viewmatrices,
+                           const float* projmatrices, const float* cam_poses, const float* tan_fovx_host,
+                           const float* tan_fovy_host, int prefiltered, float* out_color, int* radii,
+                           float* out_depth, float* out_alpha, const float* normals, int normals_per_frame,
+                           float* out_normal, void* nrm_ws, size_t nrm_ws_stride, float near_, float far_,
+                           float* out_median, float* out_distortion, void* surf_ws, size_t surf_ws_stride,
+                           void* geom_ws, size_t geom_stride, void* binning_ws, size_t binning_stride,
+                           int64_t R_cap, void* img_ws, size_t img_stride, int32_t* status, int32_t* status_host,
+                           void* status_event, float depth_hint_lo, float depth_hint_hi, int max_tile_hint,
+                           int n_streams, void* stream) {
+  if (F <= 0 || !tan_fovx_host || !tan_fovy_host || !viewmatrices || !projmatrices || !cam_poses)
+    return bad("dgr_forward_batch: bad argument");
+  size_t gb, bb, ib;
+  if (dgr_workspace_sizes(P, W, H, R_cap, &gb, &bb, &ib) != DGM_OK) return DGM_E_BADARG;
+  if (geom_stride < gb || binning_stride < bb || img_stride < ib || (geom_stride | binning_stride | img_stride) & 127) {
+    strncpy(g_last_error, "dgr_forward_batch: workspace stride too small / unaligned", sizeof(g_last_error) - 1);
+    return DGM_E_WORKSPACE;
+  }
+  int rc;
+  if (out_normal) {
+    if ((rc = normal_args(P, R_cap, normals, out_normal, nrm_ws, nrm_ws_stride)) != DGM_OK) return rc;
+    if (nrm_ws_stride & 127) return bad("dgr_forward_batch_nrm: normal workspace stride unaligned");
+  }
+  if (out_median || out_distortion) {
+    if ((rc = surface_args(W, H, near_, far_, surf_ws, surf_ws_stride)) != DGM_OK) return rc;
+    if (surf_ws_stride & 127) return bad("dgr_forward_batch_surf: surface workspace stride unaligned");
+  }
+  if (!background || !out_color || !status) return bad("dgr_forward_batch: null required pointer");
+  if (P > 0) {
+    rc = gaussian_args("dgr_forward_batch", D, M, means3D, shs, colors_precomp, opacities, scales, rotations,
+                       cov3D_precomp);
+    if (rc != DGM_OK) return rc;
+    if (!geom_ws || !binning_ws || !img_ws) {
+      strncpy(g_last_error, "dgr_forward_batch: workspace missing", sizeof(g_last_error) - 1);
+      return DGM_E_WORKSPACE;
+    }
+  }
+  return forward_frames(F, P, D, M, background, W, H, means3D, shs, colors_precomp, opacities, scales, scale_modifier,
+                        rotations, cov3D_precomp, per_frame, viewmatrices, projmatrices, cam_poses, tan_fovx_host,
+                        tan_fovy_host, prefiltered, out_color, radii, out_depth, out_alpha, normals, normals_per_frame,
+                        out_normal, nrm_ws, nrm_ws_stride, near_, far_, out_median, out_distortion, surf_ws,
+                        surf_ws_stride, geom_ws, geom_stride, binning_ws, binning_stride, R_cap, img_ws, img_stride,
+                        status, status_host, status_event, depth_hint_lo, depth_hint_hi, max_tile_hint, n_streams,
+                        stream);
+}
+
+int dgr_forward_batch_nrm(int F, int P, int D, int M, const float* background, int W, int H, const float* means3D,
+                          const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
+                          float scale_modifier, const float* rotations, const float* cov3D_precomp, int per_frame,
+                          const float* viewmatrices, const float* projmatrices, const float* cam_poses,
+                          const float* tan_fovx_host, const float* tan_fovy_host, int prefiltered, float* out_color,
+                          int* radii, float* out_depth, float* out_alpha, const float* normals, int normals_per_frame,
+                          float* out_normal, void* nrm_ws, size_t nrm_ws_stride, void* geom_ws, size_t geom_stride,
+                          void* binning_ws, size_t binning_stride, int64_t R_cap, void* img_ws, size_t img_stride,
+                          int32_t* status, int32_t* status_host, void* status_event, float depth_hint_lo,
+                          float depth_hint_hi, int max_tile_hint, int n_streams, void* stream) {
+  return dgr_forward_batch_surf(F, P, D, M, background, W, H, means3D, shs, colors_precomp, opacities, scales,
+                                scale_modifier, rotations, cov3D_precomp, per_frame, viewmatrices, projmatrices,
+                                cam_poses, tan_fovx_host, tan_fovy_host, prefiltered, out_color, radii, out_depth,
+                                out_alpha, normals, normals_per_frame, out_normal, nrm_ws, nrm_ws_stride, 0.f, 0.f,
+                                nullptr, nullptr, nullptr, 0, geom_ws, geom_stride, binning_ws, binning_stride, R_cap,
+                                img_ws, img_stride, status, status_host, status_event, depth_hint_lo, depth_hint_hi,
+                                max_tile_hint, n_streams, stream);
+}
+
+int dgr_forward_batch_aux(int F, int P, int D, int M, const float* background, int W, int H, const float* means3D,
+                          const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
+                          float scale_modifier, const float* rotations, const float* cov3D_precomp, int per_frame,
+                          const float* viewmatrices, const float* projmatrices, const float* cam_poses,
+                          const float* tan_fovx_host, const float* tan_fovy_host, int prefiltered, float* out_color,
+                          int* radii, float* out_depth, float* out_alpha, void* geom_ws, size_t geom_stride,
+                          void* binning_ws, size_t binning_stride, int64_t R_cap, void* img_ws, size_t img_stride,
+                          int32_t* status, int32_t* status_host, void* status_event, float depth_hint_lo,
+                          float depth_hint_hi, int max_tile_hint, int n_streams, void* stream) {
+  return dgr_forward_batch_nrm(F, P, D, M, background, W, H, means3D, shs, colors_precomp, opacities, scales,
+                               scale_modifier, rotations, cov3D_precomp, per_frame, viewmatrices, projmatrices,
+                               cam_poses, tan_fovx_host, tan_fovy_host, prefiltered, out_color, radii, out_depth,
+                               out_alpha, nullptr, 0, nullptr, nullptr, 0, geom_ws, geom_stride, binning_ws,
+                               binning_stride, R_cap, img_ws, img_stride, status, status_host, status_event,
+                               depth_hint_lo, depth_hint_hi, max_tile_hint, n_streams, stream);
+}
+
+int dgr_forward_batch(int F, int P, int D, int M, const float* background, int W, int H, const float* means3D,
+                      const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
+                      float scale_modifier, const float* rotations, const float* cov3D_precomp, int per_frame,
+                      const float* viewmatrices, const float* projmatrices, const float* cam_poses,
+                      const float* tan_fovx_host, const float* tan_fovy_host, int prefiltered, float* out_color,
+                      int* radii, void* geom_ws, size_t geom_stride, void* binning_ws, size_t binning_stride,
+                      int64_t R_cap, void* img_ws, size_t img_stride, int32_t* status, int32_t* status_host,
+                      void* status_event, float depth_hint_lo, float depth_hint_hi, int max_tile_hint, int n_streams,
+                      void* stream) {
+  return dgr_forward_batch_aux(F, P, D, M, background, W, H, means3D, shs, colors_precomp, opacities, scales,
+                               scale_modifier, rotations, cov3D_precomp, per_frame, viewmatrices, projmatrices,
+                               cam_poses, tan_fovx_host, tan_fovy_host, prefiltered, out_color, radii, nullptr,
+                               nullptr, geom_ws, geom_stride, binning_ws, binning_stride, R_cap, img_ws, img_stride,
+                               status, status_host, status_event, depth_hint_lo, depth_hint_hi, max_tile_hint,
+                               n_streams, stream);
 }
 
 int dgr_camera_grad_workspace_size(int F, int P, size_t* bytes) {
@@ -306,6 +524,88 @@ int camera_args(int F, int P, float* dL_dview, float* dL_dproj, float* dL_dcampo
   }
   return DGM_OK;
 }
+
+// The backward of F frames of P > 0 Gaussians whose arguments have been checked, in the layout of
+// dgr_backward_batch_abs plus the [P,4] dL_dconic of a single frame (one frame: the arguments of dgr_backward_abs
+// with F = 1, strides 0 and one stream).  Each frame's blend backward (+ median gradient), then one per-Gaussian
+// backward for all frames (+ the normal gradients) on the caller's stream.
+int backward_frames(int F, int P, int D, int M, const float* background, int W, int H, const float* means3D,
+                    const float* shs, const float* colors_precomp, const float* scales, float scale_modifier,
+                    const float* rotations, const float* cov3D_precomp, int per_frame, const float* viewmatrices,
+                    const float* projmatrices, const float* cam_poses, const float* tan_fovx_host,
+                    const float* tan_fovy_host, const int* radii, void* geom_ws, size_t geom_stride,
+                    void* binning_ws, size_t binning_stride, int64_t R_cap, void* img_ws, size_t img_stride,
+                    const float* dL_dpix, const float* dL_ddepth, const float* dL_dalpha, float* dL_dmean2D,
+                    float* dL_dconic, float* dL_dopacity, float* dL_dcolor, float* dL_dmean3D, float* dL_dcov3D,
+                    float* dL_dsh, float* dL_dscale, float* dL_drot, float* dL_dviewmatrix, float* dL_dprojmatrix,
+                    float* dL_dcampos, void* cam_ws, const float* dL_dnormal_maps, int normals_per_frame,
+                    float* dL_dnormals, void* nrm_ws, size_t nrm_ws_stride, float near_, float far_,
+                    const float* dL_dmedian, const float* dL_ddistortion, void* surf_ws, size_t surf_ws_stride,
+                    float* dL_dmean2D_abs, int n_streams, void* stream) {
+  // the render_bwd kernels alternate two low-priority streams (the next one's CTAs fill the SMs while the
+  // previous one's tail drains); one per-Gaussian kernel for all frames follows once both have finished
+  const bool multi = n_streams > 1 && F > 1;
+  cudaStream_t main_s = (cudaStream_t)stream;
+  // the kernels of every frame add into its slab: zeroed on the call's stream, before the fork
+  if (dL_dmean2D_abs) cudaMemsetAsync(dL_dmean2D_abs, 0, sizeof(float) * 3 * (size_t)F * P, main_s);
+  BatchStreams* bs = nullptr;
+  std::unique_lock<std::mutex> lk;
+  if (multi) {
+    bs = batch_streams();
+    if (!bs) return check(cudaGetLastError());
+    lk = std::unique_lock<std::mutex>(bs->mu);
+    cudaEventRecord(bs->fork, main_s);
+    for (int i = 0; i < 2; ++i) cudaStreamWaitEvent(bs->lo[i], bs->fork, 0);
+  }
+  dgm::BwdArgs a;
+  a.P = P; a.D = D; a.M = M; a.background = background; a.W = W; a.H = H;
+  a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.scales = scales;
+  a.scale_modifier = scale_modifier; a.rotations = rotations; a.cov3D_precomp = cov3D_precomp;
+  a.viewmatrix = viewmatrices; a.projmatrix = projmatrices; a.cam_pos = cam_poses;
+  a.tan_fovx = tan_fovx_host; a.tan_fovy = tan_fovy_host; a.radii = radii;
+  a.geom_ws = geom_ws; a.binning_ws = binning_ws; a.img_ws = img_ws; a.R_cap = R_cap; a.dL_dpix = dL_dpix;
+  a.dL_ddepth = dL_ddepth; a.dL_dalpha = dL_dalpha; a.dL_dmean2D = dL_dmean2D; a.dL_dconic = dL_dconic;
+  a.dL_dopacity = dL_dopacity; a.dL_dcolor = dL_dcolor; a.dL_dmean3D = dL_dmean3D; a.dL_dcov3D = dL_dcov3D;
+  a.dL_dsh = dL_dsh; a.dL_dscale = dL_dscale; a.dL_drot = dL_drot;
+  a.F = F; a.per_frame = per_frame; a.geom_stride = geom_stride;
+  a.dL_dview = dL_dviewmatrix; a.dL_dproj = dL_dprojmatrix; a.dL_dcampos = dL_dcampos; a.cam_ws = (float*)cam_ws;
+  if (dL_dnormal_maps) {
+    a.dL_dnormal = dL_dnormal_maps; a.dL_dnormals = dL_dnormals; a.nrm_ws = nrm_ws; a.nrm_stride = nrm_ws_stride;
+    a.normals_per_frame = normals_per_frame;
+  }
+  if (dL_dmedian || dL_ddistortion) {
+    a.dL_dmedian = dL_dmedian; a.dL_ddistortion = dL_ddistortion; a.surf_ws = surf_ws;
+    a.surf_k = surf_k(near_, far_);
+  }
+  cudaError_t e = cudaSuccess;
+  for (int f = 0; f < F && e == cudaSuccess; ++f) {
+    dgm::BwdArgs af = a;  // launch_render_bwd reads frame 0 of its arguments
+    af.geom_ws = (char*)geom_ws + f * geom_stride; af.binning_ws = (char*)binning_ws + f * binning_stride;
+    af.img_ws = (char*)img_ws + f * img_stride; af.dL_dpix = dL_dpix + (size_t)f * 3 * W * H;
+    if (dL_ddepth) af.dL_ddepth = dL_ddepth + (size_t)f * W * H;
+    if (dL_dalpha) af.dL_dalpha = dL_dalpha + (size_t)f * W * H;
+    if (dL_dnormal_maps) {
+      af.dL_dnormal = dL_dnormal_maps + (size_t)f * 3 * W * H;
+      af.nrm_ws = (char*)nrm_ws + f * nrm_ws_stride;
+    }
+    if (dL_dmedian) af.dL_dmedian = dL_dmedian + (size_t)f * W * H;
+    if (dL_ddistortion) af.dL_ddistortion = dL_ddistortion + (size_t)f * W * H;
+    if (a.surf_ws) af.surf_ws = (char*)surf_ws + f * surf_ws_stride;
+    if (dL_dmean2D_abs) af.dL_dmean2D_abs = dL_dmean2D_abs + (size_t)f * 3 * P;
+    cudaStream_t fs = multi ? bs->lo[f & 1] : main_s;
+    e = dgm::launch_render_bwd(af, fs);
+    if (e == cudaSuccess && dL_dmedian) e = dgm::launch_median_grad(af, fs);
+  }
+  if (multi) {
+    for (int i = 0; i < 2; ++i) {
+      cudaEventRecord(bs->done_lo[i], bs->lo[i]);
+      cudaStreamWaitEvent(main_s, bs->done_lo[i], 0);
+    }
+  }
+  if (e == cudaSuccess) e = dgm::launch_preprocess_bwd(a, main_s);
+  if (e == cudaSuccess && dL_dnormal_maps) e = dgm::launch_normal_grad_finish(a, main_s);
+  return check(e != cudaSuccess ? e : cudaGetLastError());
+}
 }  // namespace
 
 int dgr_backward_abs(int P, int D, int M, const float* background, int W, int H, const float* means3D,
@@ -320,8 +620,7 @@ int dgr_backward_abs(int P, int D, int M, const float* background, int W, int H,
                      float* dL_dnormals, void* nrm_ws, float near_, float far_, const float* dL_dmedian,
                      const float* dL_ddistortion, void* surf_ws, float* dL_dmean2D_abs, void* stream) {
   if (P < 0 || W <= 0 || H <= 0 || R_cap < 0) return bad("dgr_backward: negative size");
-  const bool surf = dL_dmedian || dL_ddistortion;
-  if (surf) {
+  if (dL_dmedian || dL_ddistortion) {
     const int rc = surface_range(near_, far_);
     if (rc != DGM_OK) return rc;
     if (!surf_ws) return bad("dgr_backward_surf: surface workspace missing");
@@ -336,29 +635,12 @@ int dgr_backward_abs(int P, int D, int M, const float* background, int W, int H,
       !dL_drot)
     return bad("dgr_backward: null required pointer");
   if (shs && !dL_dsh) return bad("dgr_backward: dL_dsh missing");
-  dgm::BwdArgs a;
-  a.P = P; a.D = D; a.M = M; a.background = background; a.W = W; a.H = H;
-  a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.scales = scales;
-  a.scale_modifier = scale_modifier; a.rotations = rotations; a.cov3D_precomp = cov3D_precomp;
-  a.viewmatrix = viewmatrix; a.projmatrix = projmatrix; a.cam_pos = cam_pos;
-  a.tan_fovx = &tan_fovx; a.tan_fovy = &tan_fovy; a.radii = radii;
-  a.geom_ws = geom_ws; a.binning_ws = binning_ws; a.img_ws = img_ws; a.R_cap = R_cap;
-  a.dL_dpix = dL_dpix; a.dL_ddepth = dL_ddepth; a.dL_dalpha = dL_dalpha;
-  a.dL_dmean2D = dL_dmean2D; a.dL_dconic = dL_dconic; a.dL_dopacity = dL_dopacity;
-  a.dL_dcolor = dL_dcolor; a.dL_dmean3D = dL_dmean3D; a.dL_dcov3D = dL_dcov3D; a.dL_dsh = dL_dsh;
-  a.dL_dscale = dL_dscale; a.dL_drot = dL_drot;
-  a.F = 1; a.per_frame = 0; a.geom_stride = 0;
-  a.dL_dview = dL_dviewmatrix; a.dL_dproj = dL_dprojmatrix; a.dL_dcampos = dL_dcampos; a.cam_ws = (float*)cam_ws;
-  if (dL_dnormal_map) a.dL_dnormal = dL_dnormal_map, a.dL_dnormals = dL_dnormals, a.nrm_ws = nrm_ws;
-  if (surf) {
-    a.dL_dmedian = dL_dmedian; a.dL_ddistortion = dL_ddistortion; a.surf_ws = surf_ws;
-    a.surf_k = surf_k(near_, far_);
-  }
-  if (dL_dmean2D_abs) {  // the kernels add into it
-    cudaMemsetAsync(dL_dmean2D_abs, 0, sizeof(float) * 3 * (size_t)P, (cudaStream_t)stream);
-    a.dL_dmean2D_abs = dL_dmean2D_abs;
-  }
-  return check(dgm::launch_backward(a, (cudaStream_t)stream));
+  return backward_frames(1, P, D, M, background, W, H, means3D, shs, colors_precomp, scales, scale_modifier, rotations,
+                         cov3D_precomp, 0, viewmatrix, projmatrix, cam_pos, &tan_fovx, &tan_fovy, radii, geom_ws, 0,
+                         binning_ws, 0, R_cap, img_ws, 0, dL_dpix, dL_ddepth, dL_dalpha, dL_dmean2D, dL_dconic,
+                         dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, dL_dviewmatrix,
+                         dL_dprojmatrix, dL_dcampos, cam_ws, dL_dnormal_map, 0, dL_dnormals, nrm_ws, 0, near_, far_,
+                         dL_dmedian, dL_ddistortion, surf_ws, 0, dL_dmean2D_abs, 1, stream);
 }
 
 int dgr_backward_surf(int P, int D, int M, const float* background, int W, int H, const float* means3D,
@@ -442,236 +724,6 @@ int dgr_backward(int P, int D, int M, const float* background, int W, int H, con
                           dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dsh, dL_dscale, dL_drot, stream);
 }
 
-namespace {
-// Internal streams for the frame batches (created once per process).
-//   hi[]  high priority: the short, latency-bound kernels (preprocess / binning / sort)
-//   lo[]  low priority : the blend kernels, each of which fills the GPU on its own; two streams,
-//         alternating frames, so the next kernel's CTAs fill the SMs while the previous one's tail drains
-// A frame's binning chain runs on hi[f % NH] and its blend kernel on lo behind an event.  The block
-// scheduler serves pending high-priority CTAs first, so the binning chains of the NEXT frames slip
-// through while the blend kernel of the current frame is running (they are latency-bound and cost
-// the issue-bound blend kernel almost nothing) instead of queueing behind its 2 500 CTAs.
-struct BatchStreams {
-  static const int NH = 4;
-  cudaStream_t hi[NH] = {}, lo[2] = {};
-  cudaEvent_t fork = nullptr, done_hi[NH] = {}, done_lo[2] = {}, ready[NH] = {};
-  bool ok = false;
-  std::mutex mu;  // one batch call at a time per device (the events above are shared)
-  bool init() {
-    if (ok) return true;
-    int least = 0, greatest = 0;
-    if (cudaDeviceGetStreamPriorityRange(&least, &greatest) != cudaSuccess) return false;
-    for (int i = 0; i < NH; ++i) {
-      if (cudaStreamCreateWithPriority(&hi[i], cudaStreamNonBlocking, greatest) != cudaSuccess) return false;
-      if (cudaEventCreateWithFlags(&done_hi[i], cudaEventDisableTiming) != cudaSuccess) return false;
-      if (cudaEventCreateWithFlags(&ready[i], cudaEventDisableTiming) != cudaSuccess) return false;
-    }
-    if (cudaEventCreateWithFlags(&fork, cudaEventDisableTiming) != cudaSuccess) return false;
-    for (int i = 0; i < 2; ++i) {
-      if (cudaStreamCreateWithPriority(&lo[i], cudaStreamNonBlocking, least) != cudaSuccess) return false;
-      if (cudaEventCreateWithFlags(&done_lo[i], cudaEventDisableTiming) != cudaSuccess) return false;
-    }
-    ok = true;
-    return true;
-  }
-};
-// one set per device, created on first use
-std::mutex g_bs_mu;
-std::map<int, BatchStreams*> g_bs_map;
-BatchStreams* batch_streams() {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
-  std::lock_guard<std::mutex> lk(g_bs_mu);
-  BatchStreams*& p = g_bs_map[dev];
-  if (!p) p = new BatchStreams();
-  return p->init() ? p : nullptr;
-}
-
-dgm::FwdArgs fwd_args(int P, int D, int M, const float* background, int W, int H, const float* means3D,
-                      const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
-                      float scale_modifier, const float* rotations, const float* cov3D_precomp,
-                      const float* viewmatrix, const float* projmatrix, const float* cam_pos, float tan_fovx,
-                      float tan_fovy, int prefiltered, float* out_color, int* radii, float* out_depth,
-                      float* out_alpha, void* geom_ws, void* binning_ws, int64_t R_cap, void* img_ws, int32_t* status,
-                      int32_t* status_host, float hint_lo, float hint_hi, int hint_max_tile) {
-  dgm::FwdArgs a;
-  a.P = P; a.D = D; a.M = M; a.background = background; a.W = W; a.H = H;
-  a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.opacities = opacities;
-  a.scales = scales; a.scale_modifier = scale_modifier; a.rotations = rotations; a.cov3D_precomp = cov3D_precomp;
-  a.viewmatrix = viewmatrix; a.projmatrix = projmatrix; a.cam_pos = cam_pos;
-  a.tan_fovx = tan_fovx; a.tan_fovy = tan_fovy; a.prefiltered = prefiltered;
-  a.out_color = out_color; a.radii = radii; a.out_depth = out_depth; a.out_alpha = out_alpha;
-  a.geom_ws = geom_ws; a.binning_ws = binning_ws; a.img_ws = img_ws; a.R_cap = R_cap; a.status = status;
-  a.status_host = status_host; a.status_event = nullptr; a.hint_lo = hint_lo; a.hint_hi = hint_hi;
-  a.hint_max_tile = hint_max_tile;
-  return a;
-}
-}  // namespace
-
-int dgr_forward_batch_surf(int F, int P, int D, int M, const float* background, int W, int H,
-                           const float* means3D, const float* shs, const float* colors_precomp,
-                           const float* opacities, const float* scales, float scale_modifier, const float* rotations,
-                           const float* cov3D_precomp, int per_frame, const float* viewmatrices,
-                           const float* projmatrices, const float* cam_poses, const float* tan_fovx_host,
-                           const float* tan_fovy_host, int prefiltered, float* out_color, int* radii,
-                           float* out_depth, float* out_alpha, const float* normals, int normals_per_frame,
-                           float* out_normal, void* nrm_ws, size_t nrm_ws_stride, float near_, float far_,
-                           float* out_median, float* out_distortion, void* surf_ws, size_t surf_ws_stride,
-                           void* geom_ws, size_t geom_stride, void* binning_ws, size_t binning_stride,
-                           int64_t R_cap, void* img_ws, size_t img_stride, int32_t* status, int32_t* status_host,
-                           void* status_event, float depth_hint_lo, float depth_hint_hi, int max_tile_hint,
-                           int n_streams, void* stream) {
-  if (F <= 0 || !tan_fovx_host || !tan_fovy_host || !viewmatrices || !projmatrices || !cam_poses)
-    return bad("dgr_forward_batch: bad argument");
-  size_t gb, bb, ib;
-  if (dgr_workspace_sizes(P, W, H, R_cap, &gb, &bb, &ib) != DGM_OK) return DGM_E_BADARG;
-  if (geom_stride < gb || binning_stride < bb || img_stride < ib || (geom_stride | binning_stride | img_stride) & 127) {
-    strncpy(g_last_error, "dgr_forward_batch: workspace stride too small / unaligned", sizeof(g_last_error) - 1);
-    return DGM_E_WORKSPACE;
-  }
-  if (out_normal) {
-    const int rc = normal_args(P, R_cap, normals, out_normal, nrm_ws, nrm_ws_stride);
-    if (rc != DGM_OK) return rc;
-    if (nrm_ws_stride & 127) return bad("dgr_forward_batch_nrm: normal workspace stride unaligned");
-  }
-  const bool surf = out_median || out_distortion;
-  if (surf) {
-    const int rc = surface_args(W, H, near_, far_, surf_ws, surf_ws_stride);
-    if (rc != DGM_OK) return rc;
-    if (surf_ws_stride & 127) return bad("dgr_forward_batch_surf: surface workspace stride unaligned");
-  }
-  // frame f's surface maps and surface workspace
-  auto srf_w = [&](int f) { return surf ? (void*)((char*)surf_ws + f * surf_ws_stride) : nullptr; };
-  // frame f's normals ([F,P,3] with normals_per_frame), normal map and normal workspace
-  auto nrm_in = [&](int f) { return (normals && normals_per_frame) ? normals + (size_t)f * P * 3 : normals; };
-  auto nrm_out = [&](int f) { return out_normal ? out_normal + (size_t)f * 3 * W * H : out_normal; };
-  auto nrm_w = [&](int f) { return nrm_ws ? (void*)((char*)nrm_ws + f * nrm_ws_stride) : nullptr; };
-  cudaStream_t main_s = (cudaStream_t)stream;
-  const bool multi = n_streams > 1 && F > 1 && P > 0;
-  const int NH = multi ? (n_streams > BatchStreams::NH ? BatchStreams::NH : n_streams) : 0;
-  // per-frame inputs (bit set in per_frame) advance by one [P, .] slab per frame
-  auto pf = [&](const float* p, int bit, size_t width, int f) {
-    return (p && (per_frame & bit)) ? p + (size_t)f * P * width : p;
-  };
-  const size_t cw = shs ? (size_t)M * 3 : 3;
-  auto map = [&](float* p, int f) { return p ? p + (size_t)f * W * H : p; };  // frame f of an [F,H,W] map
-  if (!multi) {
-    int rc = DGM_OK;
-    for (int f = 0; f < F && rc == DGM_OK; ++f)
-      rc = forward_one(P, D, M, background, W, H, pf(means3D, DGR_PF_MEANS, 3, f), pf(shs, DGR_PF_COLOR, cw, f),
-                       pf(colors_precomp, DGR_PF_COLOR, 3, f), pf(opacities, DGR_PF_OPAC, 1, f),
-                       pf(scales, DGR_PF_SCALES, 3, f), scale_modifier, pf(rotations, DGR_PF_ROTS, 4, f),
-                       pf(cov3D_precomp, DGR_PF_COV, 6, f), viewmatrices + 16 * f, projmatrices + 16 * f,
-                       cam_poses + 3 * f, tan_fovx_host[f], tan_fovy_host[f], prefiltered,
-                       out_color + (size_t)f * 3 * W * H, radii ? radii + (size_t)f * P : nullptr, map(out_depth, f),
-                       map(out_alpha, f), nrm_in(f), nrm_out(f), nrm_w(f), nrm_ws_stride, near_, far_,
-                       map(out_median, f), map(out_distortion, f), srf_w(f), surf_ws_stride, (char*)geom_ws + f * geom_stride, geom_stride, (char*)binning_ws + f * binning_stride,
-                       binning_stride, R_cap, (char*)img_ws + f * img_stride, img_stride, status + f * DGR_STATUS_WORDS,
-                       status_host ? status_host + f * DGR_STATUS_WORDS : nullptr,
-                       (f == F - 1) ? status_event : nullptr, depth_hint_lo, depth_hint_hi, max_tile_hint, main_s);
-    return rc;
-  }
-  if (!background || !out_color || !status || !means3D || !opacities) return bad("dgr_forward_batch: null required pointer");
-  if ((shs == nullptr) == (colors_precomp == nullptr)) return bad("dgr_forward_batch: exactly one of shs / colors_precomp");
-  if (((scales == nullptr) || (rotations == nullptr)) == (cov3D_precomp == nullptr))
-    return bad("dgr_forward_batch: exactly one of scales+rotations / cov3D_precomp");
-  if (shs && (M <= 0 || M > 16 || (D + 1) * (D + 1) > M || D < 0 || D > 3))
-    return bad("dgr_forward_batch: SH degree / coefficient count");
-  BatchStreams* bs = batch_streams();
-  if (!bs) return check(cudaGetLastError());
-  std::lock_guard<std::mutex> lk(bs->mu);
-  cudaEventRecord(bs->fork, main_s);
-  for (int i = 0; i < NH; ++i) cudaStreamWaitEvent(bs->hi[i], bs->fork, 0);
-  for (int i = 0; i < 2; ++i) cudaStreamWaitEvent(bs->lo[i], bs->fork, 0);
-  cudaError_t e = cudaSuccess;
-  for (int f = 0; f < F && e == cudaSuccess; ++f) {
-    const int i = f % NH;
-    cudaStream_t lo = bs->lo[f & 1];
-    dgm::FwdArgs a = fwd_args(
-        P, D, M, background, W, H, pf(means3D, DGR_PF_MEANS, 3, f), pf(shs, DGR_PF_COLOR, cw, f),
-        pf(colors_precomp, DGR_PF_COLOR, 3, f), pf(opacities, DGR_PF_OPAC, 1, f), pf(scales, DGR_PF_SCALES, 3, f),
-        scale_modifier, pf(rotations, DGR_PF_ROTS, 4, f), pf(cov3D_precomp, DGR_PF_COV, 6, f), viewmatrices + 16 * f,
-        projmatrices + 16 * f, cam_poses + 3 * f, tan_fovx_host[f], tan_fovy_host[f], prefiltered,
-        out_color + (size_t)f * 3 * W * H, radii ? radii + (size_t)f * P : nullptr, map(out_depth, f),
-        map(out_alpha, f), (char*)geom_ws + f * geom_stride,
-        (char*)binning_ws + f * binning_stride, R_cap, (char*)img_ws + f * img_stride, status + f * DGR_STATUS_WORDS,
-        status_host ? status_host + f * DGR_STATUS_WORDS : nullptr, depth_hint_lo, depth_hint_hi, max_tile_hint);
-    if (out_normal) a.normals = nrm_in(f), a.out_normal = nrm_out(f), a.nrm_ws = nrm_w(f);
-    if (surf) {
-      a.out_median = map(out_median, f); a.out_distortion = map(out_distortion, f); a.surf_ws = srf_w(f);
-      a.surf_k = surf_k(near_, far_);
-    }
-    e = dgm::launch_binning(a, bs->hi[i]);
-    cudaEventRecord(bs->ready[i], bs->hi[i]);
-    cudaStreamWaitEvent(lo, bs->ready[i], 0);
-    if (e == cudaSuccess) e = dgm::launch_render(a, lo);
-  }
-  // the binning chains finish long before the blend kernels: the caller's status event fires then
-  for (int i = 0; i < NH; ++i) {
-    cudaEventRecord(bs->done_hi[i], bs->hi[i]);
-    cudaStreamWaitEvent(main_s, bs->done_hi[i], 0);
-  }
-  if (status_event) cudaEventRecord((cudaEvent_t)status_event, main_s);
-  for (int i = 0; i < 2; ++i) {
-    cudaEventRecord(bs->done_lo[i], bs->lo[i]);
-    cudaStreamWaitEvent(main_s, bs->done_lo[i], 0);
-  }
-  return check(e != cudaSuccess ? e : cudaGetLastError());
-}
-
-int dgr_forward_batch_nrm(int F, int P, int D, int M, const float* background, int W, int H, const float* means3D,
-                          const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
-                          float scale_modifier, const float* rotations, const float* cov3D_precomp, int per_frame,
-                          const float* viewmatrices, const float* projmatrices, const float* cam_poses,
-                          const float* tan_fovx_host, const float* tan_fovy_host, int prefiltered, float* out_color,
-                          int* radii, float* out_depth, float* out_alpha, const float* normals, int normals_per_frame,
-                          float* out_normal, void* nrm_ws, size_t nrm_ws_stride, void* geom_ws, size_t geom_stride,
-                          void* binning_ws, size_t binning_stride, int64_t R_cap, void* img_ws, size_t img_stride,
-                          int32_t* status, int32_t* status_host, void* status_event, float depth_hint_lo,
-                          float depth_hint_hi, int max_tile_hint, int n_streams, void* stream) {
-  return dgr_forward_batch_surf(F, P, D, M, background, W, H, means3D, shs, colors_precomp, opacities, scales,
-                                scale_modifier, rotations, cov3D_precomp, per_frame, viewmatrices, projmatrices,
-                                cam_poses, tan_fovx_host, tan_fovy_host, prefiltered, out_color, radii, out_depth,
-                                out_alpha, normals, normals_per_frame, out_normal, nrm_ws, nrm_ws_stride, 0.f, 0.f,
-                                nullptr, nullptr, nullptr, 0, geom_ws, geom_stride, binning_ws, binning_stride, R_cap,
-                                img_ws, img_stride, status, status_host, status_event, depth_hint_lo, depth_hint_hi,
-                                max_tile_hint, n_streams, stream);
-}
-
-int dgr_forward_batch_aux(int F, int P, int D, int M, const float* background, int W, int H, const float* means3D,
-                          const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
-                          float scale_modifier, const float* rotations, const float* cov3D_precomp, int per_frame,
-                          const float* viewmatrices, const float* projmatrices, const float* cam_poses,
-                          const float* tan_fovx_host, const float* tan_fovy_host, int prefiltered, float* out_color,
-                          int* radii, float* out_depth, float* out_alpha, void* geom_ws, size_t geom_stride,
-                          void* binning_ws, size_t binning_stride, int64_t R_cap, void* img_ws, size_t img_stride,
-                          int32_t* status, int32_t* status_host, void* status_event, float depth_hint_lo,
-                          float depth_hint_hi, int max_tile_hint, int n_streams, void* stream) {
-  return dgr_forward_batch_nrm(F, P, D, M, background, W, H, means3D, shs, colors_precomp, opacities, scales,
-                               scale_modifier, rotations, cov3D_precomp, per_frame, viewmatrices, projmatrices,
-                               cam_poses, tan_fovx_host, tan_fovy_host, prefiltered, out_color, radii, out_depth,
-                               out_alpha, nullptr, 0, nullptr, nullptr, 0, geom_ws, geom_stride, binning_ws,
-                               binning_stride, R_cap, img_ws, img_stride, status, status_host, status_event,
-                               depth_hint_lo, depth_hint_hi, max_tile_hint, n_streams, stream);
-}
-
-int dgr_forward_batch(int F, int P, int D, int M, const float* background, int W, int H, const float* means3D,
-                      const float* shs, const float* colors_precomp, const float* opacities, const float* scales,
-                      float scale_modifier, const float* rotations, const float* cov3D_precomp, int per_frame,
-                      const float* viewmatrices, const float* projmatrices, const float* cam_poses,
-                      const float* tan_fovx_host, const float* tan_fovy_host, int prefiltered, float* out_color,
-                      int* radii, void* geom_ws, size_t geom_stride, void* binning_ws, size_t binning_stride,
-                      int64_t R_cap, void* img_ws, size_t img_stride, int32_t* status, int32_t* status_host,
-                      void* status_event, float depth_hint_lo, float depth_hint_hi, int max_tile_hint, int n_streams,
-                      void* stream) {
-  return dgr_forward_batch_aux(F, P, D, M, background, W, H, means3D, shs, colors_precomp, opacities, scales,
-                               scale_modifier, rotations, cov3D_precomp, per_frame, viewmatrices, projmatrices,
-                               cam_poses, tan_fovx_host, tan_fovy_host, prefiltered, out_color, radii, nullptr,
-                               nullptr, geom_ws, geom_stride, binning_ws, binning_stride, R_cap, img_ws, img_stride,
-                               status, status_host, status_event, depth_hint_lo, depth_hint_hi, max_tile_hint,
-                               n_streams, stream);
-}
-
 int dgr_backward_batch_abs(int F, int P, int D, int M, const float* background, int W, int H,
                            const float* means3D, const float* shs, const float* colors_precomp, const float* scales,
                            float scale_modifier, const float* rotations, const float* cov3D_precomp, int per_frame,
@@ -707,69 +759,13 @@ int dgr_backward_batch_abs(int F, int P, int D, int M, const float* background, 
       !geom_ws || !binning_ws || !img_ws || !dL_dpix || !dL_dmean2D || !dL_dopacity || (!shs && !dL_dcolor) ||
       !dL_dmean3D || (cov3D_precomp && !dL_dcov3D) || !dL_dscale || !dL_drot || (shs && !dL_dsh))
     return bad("dgr_backward_batch: null required pointer");
-  // the render_bwd kernels alternate two low-priority streams (the next one's CTAs fill the SMs while the
-  // previous one's tail drains); one per-Gaussian kernel for all frames follows once both have finished
-  const bool multi = n_streams > 1 && F > 1;
-  cudaStream_t main_s = (cudaStream_t)stream;
-  // the kernels of every frame add into its slab: zeroed on the call's stream, before the fork
-  if (dL_dmean2D_abs) cudaMemsetAsync(dL_dmean2D_abs, 0, sizeof(float) * 3 * (size_t)F * P, main_s);
-  BatchStreams* bs = nullptr;
-  std::unique_lock<std::mutex> lk;
-  if (multi) {
-    bs = batch_streams();
-    if (!bs) return check(cudaGetLastError());
-    lk = std::unique_lock<std::mutex>(bs->mu);
-    cudaEventRecord(bs->fork, main_s);
-    for (int i = 0; i < 2; ++i) cudaStreamWaitEvent(bs->lo[i], bs->fork, 0);
-  }
-  dgm::BwdArgs a;
-  a.P = P; a.D = D; a.M = M; a.background = background; a.W = W; a.H = H;
-  a.means3D = means3D; a.shs = shs; a.colors_precomp = colors_precomp; a.scales = scales;
-  a.scale_modifier = scale_modifier; a.rotations = rotations; a.cov3D_precomp = cov3D_precomp;
-  a.viewmatrix = viewmatrices; a.projmatrix = projmatrices; a.cam_pos = cam_poses;
-  a.tan_fovx = tan_fovx_host; a.tan_fovy = tan_fovy_host; a.radii = radii;
-  a.geom_ws = geom_ws; a.binning_ws = binning_ws; a.img_ws = img_ws; a.R_cap = R_cap; a.dL_dpix = dL_dpix;
-  a.dL_ddepth = dL_ddepth; a.dL_dalpha = dL_dalpha; a.dL_dmean2D = dL_dmean2D; a.dL_dconic = nullptr; a.dL_dopacity = dL_dopacity; a.dL_dcolor = dL_dcolor;
-  a.dL_dmean3D = dL_dmean3D; a.dL_dcov3D = dL_dcov3D; a.dL_dsh = dL_dsh;
-  a.dL_dscale = dL_dscale; a.dL_drot = dL_drot;
-  a.F = F; a.per_frame = per_frame; a.geom_stride = geom_stride;
-  a.dL_dview = dL_dviewmatrix; a.dL_dproj = dL_dprojmatrix; a.dL_dcampos = dL_dcampos; a.cam_ws = (float*)cam_ws;
-  if (dL_dnormal_maps) {
-    a.dL_dnormal = dL_dnormal_maps; a.dL_dnormals = dL_dnormals; a.nrm_ws = nrm_ws; a.nrm_stride = nrm_ws_stride;
-    a.normals_per_frame = normals_per_frame;
-  }
-  if (surf) {
-    a.dL_dmedian = dL_dmedian; a.dL_ddistortion = dL_ddistortion; a.surf_ws = surf_ws;
-    a.surf_k = surf_k(near_, far_);
-  }
-  cudaError_t e = cudaSuccess;
-  for (int f = 0; f < F && e == cudaSuccess; ++f) {
-    dgm::BwdArgs af = a;  // launch_render_bwd reads frame 0 of its arguments
-    af.geom_ws = (char*)geom_ws + f * geom_stride; af.binning_ws = (char*)binning_ws + f * binning_stride;
-    af.img_ws = (char*)img_ws + f * img_stride; af.dL_dpix = dL_dpix + (size_t)f * 3 * W * H;
-    if (dL_ddepth) af.dL_ddepth = dL_ddepth + (size_t)f * W * H;
-    if (dL_dalpha) af.dL_dalpha = dL_dalpha + (size_t)f * W * H;
-    if (dL_dnormal_maps) {
-      af.dL_dnormal = dL_dnormal_maps + (size_t)f * 3 * W * H;
-      af.nrm_ws = (char*)nrm_ws + f * nrm_ws_stride;
-    }
-    if (dL_dmedian) af.dL_dmedian = dL_dmedian + (size_t)f * W * H;
-    if (dL_ddistortion) af.dL_ddistortion = dL_ddistortion + (size_t)f * W * H;
-    if (surf) af.surf_ws = (char*)surf_ws + f * surf_ws_stride;
-    if (dL_dmean2D_abs) af.dL_dmean2D_abs = dL_dmean2D_abs + (size_t)f * 3 * P;
-    cudaStream_t fs = multi ? bs->lo[f & 1] : main_s;
-    e = dgm::launch_render_bwd(af, fs);
-    if (e == cudaSuccess && dL_dmedian) e = dgm::launch_median_grad(af, fs);
-  }
-  if (multi) {
-    for (int i = 0; i < 2; ++i) {
-      cudaEventRecord(bs->done_lo[i], bs->lo[i]);
-      cudaStreamWaitEvent(main_s, bs->done_lo[i], 0);
-    }
-  }
-  if (e == cudaSuccess) e = dgm::launch_preprocess_bwd(a, main_s);
-  if (e == cudaSuccess && dL_dnormal_maps) e = dgm::launch_normal_grad_finish(a, main_s);
-  return check(e != cudaSuccess ? e : cudaGetLastError());
+  return backward_frames(F, P, D, M, background, W, H, means3D, shs, colors_precomp, scales, scale_modifier, rotations,
+                         cov3D_precomp, per_frame, viewmatrices, projmatrices, cam_poses, tan_fovx_host, tan_fovy_host,
+                         radii, geom_ws, geom_stride, binning_ws, binning_stride, R_cap, img_ws, img_stride, dL_dpix,
+                         dL_ddepth, dL_dalpha, dL_dmean2D, nullptr, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D,
+                         dL_dsh, dL_dscale, dL_drot, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, cam_ws,
+                         dL_dnormal_maps, normals_per_frame, dL_dnormals, nrm_ws, nrm_ws_stride, near_, far_,
+                         dL_dmedian, dL_ddistortion, surf_ws, surf_ws_stride, dL_dmean2D_abs, n_streams, stream);
 }
 
 int dgr_backward_batch_surf(int F, int P, int D, int M, const float* background, int W, int H,

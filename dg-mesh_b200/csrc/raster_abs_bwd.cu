@@ -5,8 +5,9 @@
 //                                     + normal map, + surface maps, + both) that also adds, per Gaussian, the sums
 //                                     over pixels of |dL/dmean2D.x| and |dL/dmean2D.y| of each pixel's term
 //
-// Kept apart from raster_bwd.cu, raster_nrm_bwd.cu and raster_surf_bwd.cu so that the kernels there compile exactly
-// as they do without the statistic.
+// launch_render_bwd_abs picks one of the five and launches it through launch_blend_bwd (raster_bwd_blend.cuh).  Kept
+// apart from raster_bwd.cu, raster_nrm_bwd.cu and raster_surf_bwd.cu so that the kernels there compile exactly as they
+// do without the statistic.
 #include "../../include/dgmesh_b200.h"
 #include "common.cuh"
 #include "raster_kernels.h"
@@ -14,52 +15,14 @@
 
 namespace dgm {
 
-namespace {
-template <bool AUX, bool NRM, bool SURF> constexpr size_t abs_smem() {
-  return (NRM || SURF) ? (size_t)DynSmem<NRM, SURF, true>::BYTES : (size_t)STAGE_BYTES;
-}
-}  // namespace
-
-// the blend backward of one frame with a.dL_dmean2D_abs (launch_render_bwd); the other arguments select the
-// instance as launch_render_bwd{,_nrm,_surf} do
+// the blend backward of one frame with a.dL_dmean2D_abs (launch_render_bwd); the other arguments pick the instance
+// by the rule of launch_blend_bwd
 cudaError_t launch_render_bwd_abs(const BwdArgs& a, cudaStream_t s) {
-  auto col = render_bwd_kernel<false, false, false, true>, aux = render_bwd_kernel<true, false, false, true>;
-  auto nrm = render_bwd_kernel<true, true, false, true>, srf = render_bwd_kernel<true, false, true, true>;
-  auto nrm_srf = render_bwd_kernel<true, true, true, true>;
-  static unsigned long long attr = 0;  // per device
-  if (once_per_device(attr)) {
-    cudaFuncSetAttribute(col, cudaFuncAttributeMaxDynamicSharedMemorySize, abs_smem<false, false, false>());
-    cudaFuncSetAttribute(aux, cudaFuncAttributeMaxDynamicSharedMemorySize, abs_smem<true, false, false>());
-    cudaFuncSetAttribute(nrm, cudaFuncAttributeMaxDynamicSharedMemorySize, abs_smem<true, true, false>());
-    cudaFuncSetAttribute(srf, cudaFuncAttributeMaxDynamicSharedMemorySize, abs_smem<true, false, true>());
-    cudaFuncSetAttribute(nrm_srf, cudaFuncAttributeMaxDynamicSharedMemorySize, abs_smem<true, true, true>());
-    for (auto k : {col, aux, nrm, srf, nrm_srf})
-      cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  }
-  if (a.P == 0) return cudaSuccess;
-  const unsigned gx = (a.W + TILE_X - 1) / TILE_X, gy = (a.H + TILE_Y - 1) / TILE_Y;
-  const int T = gx * gy;
-  GeomWS g = GeomWS::from((char*)a.geom_ws, a.P);
-  ImgWS im = ImgWS::from((char*)a.img_ws, (size_t)a.W * a.H, T);
-  BinWS b = BinWS::from((char*)a.binning_ws, (size_t)a.R_cap);
-  const bool surf = a.dL_ddistortion != nullptr, has_nrm = a.dL_dnormal != nullptr;
-  const bool has_aux = a.dL_ddepth || a.dL_dalpha || has_nrm || surf;
-  NrmWS n = {};
-  if (has_nrm) n = NrmWS::from((char*)a.nrm_ws, a.P, (size_t)a.R_cap);
-  SurfWS sw = {};
-  if (surf) sw = SurfWS::from((char*)a.surf_ws, (size_t)a.W * a.H);
-  auto k = surf ? (has_nrm ? nrm_srf : srf) : has_nrm ? nrm : has_aux ? aux : col;
-  const size_t smem = surf ? (has_nrm ? abs_smem<true, true, true>() : abs_smem<true, false, true>())
-                      : has_nrm ? abs_smem<true, true, false>()
-                                : abs_smem<false, false, false>();
-  g_prof.begin(5, s);
-  launch_pdl(k, dim3(T), dim3(256), smem, s, (const uint2*)im.ranges, (const uint32_t*)im.tile_order,
-             (const float4*)b.inst_geo, (const float4*)b.inst_attr, a.W, a.H, a.background, (const float*)im.final_T,
-             (const uint32_t*)im.n_contrib, a.dL_dpix, g.grad_acc, a.dL_ddepth, a.dL_dalpha, a.dL_dnormal,
-             (const float4*)n.inst_nrm, n.acc, a.dL_ddistortion, (const float2*)sw.moments, a.surf_k,
-             a.dL_dmean2D_abs);
-  g_prof.end(5, s);
-  return cudaGetLastError();
+  if (a.dL_ddistortion)
+    return a.dL_dnormal ? launch_blend_bwd<true, true, true, true>(a, s) : launch_blend_bwd<true, false, true, true>(a, s);
+  if (a.dL_dnormal) return launch_blend_bwd<true, true, false, true>(a, s);
+  return (a.dL_ddepth || a.dL_dalpha) ? launch_blend_bwd<true, false, false, true>(a, s)
+                                      : launch_blend_bwd<false, false, false, true>(a, s);
 }
 
 }  // namespace dgm

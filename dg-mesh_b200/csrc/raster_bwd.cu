@@ -21,9 +21,11 @@
 // reference's back-to-front recurrence; only the summation order differs (the
 // reference's own order is non-deterministic).
 //
-// render_bwd_kernel itself is in raster_bwd_blend.cuh; its normal-map instance and normal_grad_finish_kernel are
-// compiled in raster_nrm_bwd.cu, its median-depth / distortion instances and median_grad_kernel in
-// raster_surf_bwd.cu, its instances with the absolute screen-space gradient in raster_abs_bwd.cu.
+// render_bwd_kernel and its one launcher, launch_blend_bwd, are in raster_bwd_blend.cuh.  This file compiles the
+// colour-only and depth/alpha instances; the normal-map instance and normal_grad_finish_kernel are compiled in
+// raster_nrm_bwd.cu, the median-depth / distortion instances and median_grad_kernel in raster_surf_bwd.cu, the
+// instances with the absolute screen-space gradient in raster_abs_bwd.cu.  launch_render_bwd below picks the instance
+// and hands the call to the file that holds it.
 #include "../../include/dgmesh_b200.h"
 #include "common.cuh"
 #include "raster_math.cuh"
@@ -608,42 +610,14 @@ __global__ void __launch_bounds__(32 * CAM_TERMS) camera_grad_finish_kernel(int 
   }
 }
 
-cudaError_t launch_backward(const BwdArgs& a, cudaStream_t s) {
-  cudaError_t e = launch_render_bwd(a, s);
-  if (e == cudaSuccess && a.dL_dmedian) e = launch_median_grad(a, s);
-  if (e == cudaSuccess) e = launch_preprocess_bwd(a, s);
-  return (e != cudaSuccess || !a.dL_dnormal) ? e : launch_normal_grad_finish(a, s);
-}
-
-// gradient of the alpha-compositing (fills the GPU); leaves the per-Gaussian moments in grad_acc
+// gradient of the alpha-compositing (fills the GPU); leaves the per-Gaussian moments in grad_acc.  The instance follows
+// the rule of launch_blend_bwd
 cudaError_t launch_render_bwd(const BwdArgs& a, cudaStream_t s) {
   if (a.dL_dmean2D_abs) return launch_render_bwd_abs(a, s);  // raster_abs_bwd.cu
   if (a.dL_ddistortion) return launch_render_bwd_surf(a, s);  // raster_surf_bwd.cu
   if (a.dL_dnormal) return launch_render_bwd_nrm(a, s);  // raster_nrm_bwd.cu
-  static unsigned long long attr = 0;  // per device
-  if (once_per_device(attr)) {
-    // the staging area takes the kernel past 48 KB of shared memory; 3 CTAs per SM need the largest carveout
-    for (auto k : {render_bwd_kernel<false>, render_bwd_kernel<true>}) {
-      cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, STAGE_BYTES);
-      cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    }
-  }
-  if (a.P == 0) return cudaSuccess;
-  const unsigned gx = (a.W + TILE_X - 1) / TILE_X, gy = (a.H + TILE_Y - 1) / TILE_Y;
-  const int T = gx * gy;
-  GeomWS g = GeomWS::from((char*)a.geom_ws, a.P);
-  ImgWS im = ImgWS::from((char*)a.img_ws, (size_t)a.W * a.H, T);
-  BinWS b = BinWS::from((char*)a.binning_ws, (size_t)a.R_cap);
-  const bool aux = a.dL_ddepth || a.dL_dalpha;
-  g_prof.begin(5, s);
-  launch_pdl(aux ? render_bwd_kernel<true> : render_bwd_kernel<false>, dim3(T), dim3(256), STAGE_BYTES, s,
-             (const uint2*)im.ranges, (const uint32_t*)im.tile_order, (const float4*)b.inst_geo,
-             (const float4*)b.inst_attr, a.W, a.H, a.background, (const float*)im.final_T,
-             (const uint32_t*)im.n_contrib, a.dL_dpix, g.grad_acc, a.dL_ddepth, a.dL_dalpha, (const float*)nullptr,
-             (const float4*)nullptr, (float4*)nullptr, (const float*)nullptr, (const float2*)nullptr, 0.f,
-             (float*)nullptr);
-  g_prof.end(5, s);
-  return cudaGetLastError();
+  return (a.dL_ddepth || a.dL_dalpha) ? launch_blend_bwd<true, false, false, false>(a, s)
+                                      : launch_blend_bwd<false, false, false, false>(a, s);
 }
 
 // chain rule from the moments to the inputs, all frames of a batch in one launch (after every frame's

@@ -1,11 +1,12 @@
-// raster_bwd_blend.cuh -- the blend backward kernel (render_bwd_kernel) of the tile-based 3D-Gaussian rasterizer,
-// shared by raster_bwd.cu (the colour-only and depth/alpha instances), raster_nrm_bwd.cu (the normal-map
-// instance), raster_surf_bwd.cu (the median-depth / distortion instances) and raster_abs_bwd.cu (the instances with
-// the absolute screen-space gradient), each in its own translation unit so that the other kernels of raster_bwd.cu
-// compile as they did without them.
+// raster_bwd_blend.cuh -- the blend backward kernel (render_bwd_kernel) of the tile-based 3D-Gaussian rasterizer and
+// its launcher (launch_blend_bwd), shared by raster_bwd.cu (the colour-only and depth/alpha instances),
+// raster_nrm_bwd.cu (the normal-map instance), raster_surf_bwd.cu (the median-depth / distortion instances) and
+// raster_abs_bwd.cu (the instances with the absolute screen-space gradient), each in its own translation unit so that
+// the other kernels of raster_bwd.cu compile as they did without them.
 // See raster_bwd.cu for the design of the kernel.
 #pragma once
 #include "common.cuh"
+#include "raster_kernels.h"
 #include "raster_math.cuh"
 
 namespace dgm {
@@ -36,7 +37,6 @@ template <bool NRM, bool SURF = false, bool ABS = false> struct DynSmem {
   static constexpr int REC = REF + (SURF ? 4 : 0);                         // s_nrm [2][RB] float4 (16-byte aligned)
   static constexpr int BYTES = (REC + (NRM ? 2 * RB * 4 : 0)) * 4;
 };
-#define NRM_BWD_SMEM (DynSmem<true>::BYTES)
 
 // Contract the first n staged records of a warp into s_acc.  Slot k holds w and alpha T of the 32 pixels
 // (pixel = lane of the staging warp: column lane & 7, row lane >> 3) of record `rec` (held by lanes k and
@@ -138,7 +138,7 @@ __device__ __forceinline__ void contract_chunk(const float* stage, const float* 
 // the alpha map, each NULL when the loss does not use it.  dL/d(depth_i) goes to float 9 of grad_acc.
 // NRM (with AUX): also the upstream gradient of the [3,H,W] normal map (non-NULL); the records' normals stream
 // from inst_nrm and dL/dn_i = sum over pixels of alpha_i T_i dL/dN goes to nrm_acc[id] (NrmWS::acc).  Dynamic
-// shared memory: NRM_BWD_SMEM bytes (SURF: DynSmem<NRM, true>::BYTES; the others: STAGE_BYTES).
+// shared memory: DynSmem<NRM, SURF, ABS>::BYTES with NRM or SURF, else STAGE_BYTES (launch_blend_bwd).
 // SURF (with AUX): also the upstream gradient dL/dS of the distortion map (non-NULL), with the totals {M1, M2} of the
 // surface forward (surf_mom), A = 1 - T_final and m_i = surf_m(d_i, d of the tile's first record, surf_k).  Through alpha the distortion acts as one more colour channel of
 // "colour" g_i = m_i^2 A - 2 m_i M1 + M2 and no background; through the depth, dL/dm_i = 2 (m_i S_A - S_M) with
@@ -449,6 +449,41 @@ __global__ void __launch_bounds__(256, AUX || ABS ? 2 : 3) render_bwd_kernel(
       }
     }
   }
+}
+
+// The blend backward of one frame (frame 0 of a) with render_bwd_kernel<AUX, NRM, SURF, ABS>.  launch_render_bwd picks
+// the instance: NRM = dL_dnormal, SURF = dL_ddistortion, ABS = dL_dmean2D_abs, AUX = dL_ddepth || dL_dalpha || NRM ||
+// SURF; the arguments of a map the instance does not read are NULL.  Each instance is instantiated in one translation
+// unit only (see the file comment).
+template <bool AUX, bool NRM, bool SURF, bool ABS>
+cudaError_t launch_blend_bwd(const BwdArgs& a, cudaStream_t s) {
+  auto k = render_bwd_kernel<AUX, NRM, SURF, ABS>;
+  constexpr size_t smem = (NRM || SURF) ? (size_t)DynSmem<NRM, SURF, ABS>::BYTES : (size_t)STAGE_BYTES;
+  static unsigned long long attr = 0;  // per device
+  if (once_per_device(attr)) {
+    // the staging area takes every instance past 48 KB of shared memory; 2 or 3 CTAs per SM need the largest carveout
+    cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  }
+  if (a.P == 0) return cudaSuccess;
+  const unsigned gx = (a.W + TILE_X - 1) / TILE_X, gy = (a.H + TILE_Y - 1) / TILE_Y;
+  const int T = gx * gy;
+  GeomWS g = GeomWS::from((char*)a.geom_ws, a.P);
+  ImgWS im = ImgWS::from((char*)a.img_ws, (size_t)a.W * a.H, T);
+  BinWS b = BinWS::from((char*)a.binning_ws, (size_t)a.R_cap);
+  NrmWS n = {};
+  if (NRM) n = NrmWS::from((char*)a.nrm_ws, a.P, (size_t)a.R_cap);
+  SurfWS sw = {};
+  if (SURF) sw = SurfWS::from((char*)a.surf_ws, (size_t)a.W * a.H);
+  g_prof.begin(5, s);
+  launch_pdl(k, dim3(T), dim3(256), smem, s, (const uint2*)im.ranges, (const uint32_t*)im.tile_order,
+             (const float4*)b.inst_geo, (const float4*)b.inst_attr, a.W, a.H, a.background, (const float*)im.final_T,
+             (const uint32_t*)im.n_contrib, a.dL_dpix, g.grad_acc, AUX ? a.dL_ddepth : nullptr,
+             AUX ? a.dL_dalpha : nullptr, NRM ? a.dL_dnormal : nullptr, (const float4*)n.inst_nrm, n.acc,
+             SURF ? a.dL_ddistortion : nullptr, (const float2*)sw.moments, SURF ? a.surf_k : 0.f,
+             ABS ? a.dL_dmean2D_abs : nullptr);
+  g_prof.end(5, s);
+  return cudaGetLastError();
 }
 
 }  // namespace dgm

@@ -925,53 +925,43 @@ cudaError_t launch_binning(const FwdArgs& a, cudaStream_t s) {
   g_prof.end(2, s);
   g_prof.begin(3, s);
   // (a.hint_max_tile is advisory and no longer needed: the kernel walks a tile in stage-sized runs)
-  if (a.out_normal) {  // the depth records + the normal stream; the backward's accumulator starts at zero
-    const NrmWS n = NrmWS::from((char*)a.nrm_ws, a.P, (size_t)a.R_cap);
+  // the normal map adds the normal stream to the depth records; the surface maps blend the depth records
+  const bool nrm = a.out_normal, depth = a.out_depth || a.surf_ws || nrm;
+  NrmWS n = {};
+  if (nrm) {  // the backward's accumulator starts at zero
+    n = NrmWS::from((char*)a.nrm_ws, a.P, (size_t)a.R_cap);
     cudaMemsetAsync(n.acc, 0, sizeof(float4) * (size_t)a.P, s);
-    launch_pdl(tile_sort_pack_kernel<true, true>, dim3(T), dim3(256), 0, s, (const uint2*)im.ranges,
-               (const uint32_t*)im.tile_order, b.keys, (const uint32_t*)im.hist, g, a.colors_precomp,
-               (const float*)g.depths, b, (const int32_t*)a.status, a.normals, n.inst_nrm);
-  } else {
-    const bool depth = a.out_depth || a.surf_ws;  // (the surface maps blend the depth records)
-    launch_pdl(depth ? tile_sort_pack_kernel<true> : tile_sort_pack_kernel<false>, dim3(T), dim3(256), 0, s,
-               (const uint2*)im.ranges, (const uint32_t*)im.tile_order, b.keys, (const uint32_t*)im.hist, g,
-               a.colors_precomp, depth ? (const float*)g.depths : nullptr, b, (const int32_t*)a.status,
-               (const float*)nullptr, (float4*)nullptr);
   }
+  launch_pdl(nrm ? tile_sort_pack_kernel<true, true> : depth ? tile_sort_pack_kernel<true> : tile_sort_pack_kernel<false>,
+             dim3(T), dim3(256), 0, s, (const uint2*)im.ranges, (const uint32_t*)im.tile_order, b.keys,
+             (const uint32_t*)im.hist, g, a.colors_precomp, depth ? (const float*)g.depths : nullptr, b,
+             (const int32_t*)a.status, nrm ? a.normals : nullptr, n.inst_nrm);
   g_prof.end(3, s);
   return cudaGetLastError();
 }
 
-// the alpha-compositing kernel (fills the GPU)
+// the alpha-compositing kernel (fills the GPU): render_fwd_kernel<AUX, NRM, SURF> with NRM = out_normal, SURF =
+// surf_ws, AUX = out_depth || out_alpha || NRM || SURF; the arguments of a map the instance does not write are NULL
 cudaError_t launch_render(const FwdArgs& a, cudaStream_t s) {
   const unsigned gx = (a.W + TILE_X - 1) / TILE_X, gy = (a.H + TILE_Y - 1) / TILE_Y;
   const int T = gx * gy;
   ImgWS im = ImgWS::from((char*)a.img_ws, (size_t)a.W * a.H, T);
   BinWS b = BinWS::from((char*)a.binning_ws, (size_t)a.R_cap);
-  const bool aux = a.out_depth || a.out_alpha;
+  const bool nrm = a.out_normal, surf = a.surf_ws, aux = a.out_depth || a.out_alpha || nrm || surf;
+  NrmWS n = {};
+  if (nrm) n = NrmWS::from((char*)a.nrm_ws, a.P, (size_t)a.R_cap);
+  SurfWS sw = {};
+  if (surf) sw = SurfWS::from((char*)a.surf_ws, (size_t)a.W * a.H);
+  auto k = surf ? (nrm ? render_fwd_kernel<true, true, true> : render_fwd_kernel<true, false, true>)
+           : nrm ? render_fwd_kernel<true, true>
+           : aux ? render_fwd_kernel<true>
+                 : render_fwd_kernel<false>;
   g_prof.begin(4, s);
-  if (a.surf_ws) {
-    const SurfWS sw = SurfWS::from((char*)a.surf_ws, (size_t)a.W * a.H);
-    const float4* inst_nrm = a.out_normal ? NrmWS::from((char*)a.nrm_ws, a.P, (size_t)a.R_cap).inst_nrm : nullptr;
-    launch_pdl(a.out_normal ? render_fwd_kernel<true, true, true> : render_fwd_kernel<true, false, true>, dim3(T),
-               dim3(256), 0, s, (const uint2*)im.ranges, (const uint32_t*)im.tile_order, (const float4*)b.inst_geo,
-               (const float4*)b.inst_attr, a.W, a.H, a.background, im.final_T, im.n_contrib, a.out_color,
-               (const int32_t*)a.status, a.out_depth, a.out_alpha, inst_nrm, a.out_normal, sw.median_id, sw.moments,
-               a.out_median, a.out_distortion, a.surf_k);
-  } else if (a.out_normal) {
-    const NrmWS n = NrmWS::from((char*)a.nrm_ws, a.P, (size_t)a.R_cap);
-    launch_pdl(render_fwd_kernel<true, true>, dim3(T), dim3(256), 0, s, (const uint2*)im.ranges,
-               (const uint32_t*)im.tile_order, (const float4*)b.inst_geo, (const float4*)b.inst_attr, a.W, a.H,
-               a.background, im.final_T, im.n_contrib, a.out_color, (const int32_t*)a.status, a.out_depth,
-               a.out_alpha, (const float4*)n.inst_nrm, a.out_normal, (uint32_t*)nullptr, (float2*)nullptr,
-               (float*)nullptr, (float*)nullptr, 0.f);
-  } else {
-    launch_pdl(aux ? render_fwd_kernel<true> : render_fwd_kernel<false>, dim3(T), dim3(256), 0, s,
-               (const uint2*)im.ranges, (const uint32_t*)im.tile_order, (const float4*)b.inst_geo,
-               (const float4*)b.inst_attr, a.W, a.H, a.background, im.final_T, im.n_contrib, a.out_color,
-               (const int32_t*)a.status, a.out_depth, a.out_alpha, (const float4*)nullptr, (float*)nullptr,
-               (uint32_t*)nullptr, (float2*)nullptr, (float*)nullptr, (float*)nullptr, 0.f);
-  }
+  launch_pdl(k, dim3(T), dim3(256), 0, s, (const uint2*)im.ranges, (const uint32_t*)im.tile_order,
+             (const float4*)b.inst_geo, (const float4*)b.inst_attr, a.W, a.H, a.background, im.final_T, im.n_contrib,
+             a.out_color, (const int32_t*)a.status, a.out_depth, a.out_alpha, (const float4*)n.inst_nrm, a.out_normal,
+             sw.median_id, sw.moments, surf ? a.out_median : nullptr, surf ? a.out_distortion : nullptr,
+             surf ? a.surf_k : 0.f);
   g_prof.end(4, s);
   return cudaGetLastError();
 }

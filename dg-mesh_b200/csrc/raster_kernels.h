@@ -154,8 +154,11 @@ struct Profiler {
 };
 extern Profiler g_prof;
 
+// A forward is launch_binning then launch_render (launch_forward: both on one stream).  A backward of F frames is
+// launch_render_bwd (+ launch_median_grad) per frame, then launch_preprocess_bwd (+ launch_normal_grad_finish) once.
+// launch_render_bwd picks the blend instance and calls launch_blend_bwd (raster_bwd_blend.cuh) through the entry of
+// the file that compiles that instance: launch_render_bwd_{nrm,surf,abs}.
 cudaError_t launch_forward(const FwdArgs& a, cudaStream_t s);
-cudaError_t launch_backward(const BwdArgs& a, cudaStream_t s);
 cudaError_t launch_binning(const FwdArgs& a, cudaStream_t s);
 cudaError_t launch_render(const FwdArgs& a, cudaStream_t s);
 cudaError_t launch_render_bwd(const BwdArgs& a, cudaStream_t s);

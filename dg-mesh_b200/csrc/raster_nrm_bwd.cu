@@ -4,7 +4,8 @@
 //                                  alpha_i T_i dL/dN into the normal workspace's per-Gaussian accumulator
 //   normal_grad_finish_kernel      dL/dnormals from the accumulators of every frame, which it re-zeroes
 //
-// Kept apart from raster_bwd.cu so that the kernels there compile exactly as they do without the normal map.
+// launch_render_bwd_nrm launches the blend instance through launch_blend_bwd (raster_bwd_blend.cuh).  Kept apart from
+// raster_bwd.cu so that the kernels there compile exactly as they do without the normal map.
 #include "../../include/dgmesh_b200.h"
 #include "common.cuh"
 #include "raster_kernels.h"
@@ -40,27 +41,7 @@ __global__ void __launch_bounds__(256) normal_grad_finish_kernel(int F, int P, c
 
 // the blend backward of one frame with the normal map (launch_render_bwd with a.dL_dnormal)
 cudaError_t launch_render_bwd_nrm(const BwdArgs& a, cudaStream_t s) {
-  static unsigned long long attr = 0;  // per device
-  if (once_per_device(attr)) {
-    cudaFuncSetAttribute(render_bwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, NRM_BWD_SMEM);
-    cudaFuncSetAttribute(render_bwd_kernel<true, true>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                         cudaSharedmemCarveoutMaxShared);
-  }
-  if (a.P == 0) return cudaSuccess;
-  const unsigned gx = (a.W + TILE_X - 1) / TILE_X, gy = (a.H + TILE_Y - 1) / TILE_Y;
-  const int T = gx * gy;
-  GeomWS g = GeomWS::from((char*)a.geom_ws, a.P);
-  ImgWS im = ImgWS::from((char*)a.img_ws, (size_t)a.W * a.H, T);
-  BinWS b = BinWS::from((char*)a.binning_ws, (size_t)a.R_cap);
-  const NrmWS n = NrmWS::from((char*)a.nrm_ws, a.P, (size_t)a.R_cap);
-  g_prof.begin(5, s);
-  launch_pdl(render_bwd_kernel<true, true>, dim3(T), dim3(256), NRM_BWD_SMEM, s, (const uint2*)im.ranges,
-             (const uint32_t*)im.tile_order, (const float4*)b.inst_geo, (const float4*)b.inst_attr, a.W, a.H,
-             a.background, (const float*)im.final_T, (const uint32_t*)im.n_contrib, a.dL_dpix, g.grad_acc,
-             a.dL_ddepth, a.dL_dalpha, a.dL_dnormal, (const float4*)n.inst_nrm, n.acc, (const float*)nullptr,
-             (const float2*)nullptr, 0.f, (float*)nullptr);
-  g_prof.end(5, s);
-  return cudaGetLastError();
+  return launch_blend_bwd<true, true, false, false>(a, s);
 }
 
 // after the blend backward of every frame: dL/dnormals, and the accumulators back to zero

@@ -6,8 +6,9 @@
 //   median_grad_kernel                    dL/dd of each pixel's median record: the median depth is piecewise
 //                                         constant in alpha, so its gradient reaches the depth of one record only
 //
-// Kept apart from raster_bwd.cu and raster_nrm_bwd.cu so that the kernels there compile exactly as they do without
-// the surface maps.
+// launch_render_bwd_surf picks one of the two blend instances and launches it through launch_blend_bwd
+// (raster_bwd_blend.cuh).  Kept apart from raster_bwd.cu and raster_nrm_bwd.cu so that the kernels there compile
+// exactly as they do without the surface maps.
 #include "../../include/dgmesh_b200.h"
 #include "common.cuh"
 #include "raster_kernels.h"
@@ -28,34 +29,7 @@ __global__ void __launch_bounds__(256) median_grad_kernel(int npix, const uint32
 
 // the blend backward of one frame with the distortion map (launch_render_bwd with a.dL_ddistortion)
 cudaError_t launch_render_bwd_surf(const BwdArgs& a, cudaStream_t s) {
-  static unsigned long long attr = 0;  // per device
-  if (once_per_device(attr)) {
-    cudaFuncSetAttribute(render_bwd_kernel<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         DynSmem<false, true>::BYTES);
-    cudaFuncSetAttribute(render_bwd_kernel<true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         DynSmem<true, true>::BYTES);
-    for (auto k : {render_bwd_kernel<true, false, true>, render_bwd_kernel<true, true, true>})
-      cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  }
-  if (a.P == 0) return cudaSuccess;
-  const unsigned gx = (a.W + TILE_X - 1) / TILE_X, gy = (a.H + TILE_Y - 1) / TILE_Y;
-  const int T = gx * gy;
-  GeomWS g = GeomWS::from((char*)a.geom_ws, a.P);
-  ImgWS im = ImgWS::from((char*)a.img_ws, (size_t)a.W * a.H, T);
-  BinWS b = BinWS::from((char*)a.binning_ws, (size_t)a.R_cap);
-  const SurfWS sw = SurfWS::from((char*)a.surf_ws, (size_t)a.W * a.H);
-  const bool nrm = a.dL_dnormal != nullptr;
-  NrmWS n = {};
-  if (nrm) n = NrmWS::from((char*)a.nrm_ws, a.P, (size_t)a.R_cap);
-  g_prof.begin(5, s);
-  launch_pdl(nrm ? render_bwd_kernel<true, true, true> : render_bwd_kernel<true, false, true>, dim3(T), dim3(256),
-             nrm ? (size_t)DynSmem<true, true>::BYTES : (size_t)DynSmem<false, true>::BYTES, s, (const uint2*)im.ranges,
-             (const uint32_t*)im.tile_order, (const float4*)b.inst_geo, (const float4*)b.inst_attr, a.W, a.H,
-             a.background, (const float*)im.final_T, (const uint32_t*)im.n_contrib, a.dL_dpix, g.grad_acc,
-             a.dL_ddepth, a.dL_dalpha, a.dL_dnormal, (const float4*)n.inst_nrm, n.acc, a.dL_ddistortion,
-             (const float2*)sw.moments, a.surf_k, (float*)nullptr);
-  g_prof.end(5, s);
-  return cudaGetLastError();
+  return a.dL_dnormal ? launch_blend_bwd<true, true, true, false>(a, s) : launch_blend_bwd<true, false, true, false>(a, s);
 }
 
 // dL/dmedian into the depth gradient of the median records (one frame: frame 0 of the arguments); after the frame's
