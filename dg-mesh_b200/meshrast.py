@@ -133,7 +133,7 @@ def edge_opposites(tri, n_verts):
     a, b = t, t[:, [1, 2, 0]]
     third = t[:, [2, 0, 1]].reshape(-1)
     key = (torch.minimum(a, b) * int(n_verts) + torch.maximum(a, b)).reshape(-1)
-    order = torch.argsort(key)
+    order = torch.argsort(key, stable=True)    # equal keys stay in face order: the first two users pair
     ks = key[order]
     same = ks[1:] == ks[:-1]
     # first of each run of equal keys pairs with its successor
