@@ -322,15 +322,7 @@ __global__ void __launch_bounds__(256, AUX || ABS ? 2 : 3) render_bwd_kernel(
         const int jA = k * 32 + bA, jB = k * 32 + bB;
         const float4 geA = s_geo[st][jA], geB = s_geo[st][jB];
         const float4 coA = s_attr[st][2 * jA], coB = s_attr[st][2 * jB];
-        const float2 dx2 = add2_rn(make_float2(geA.x, geB.x), npx2);
-        const float2 dy2 = add2_rn(make_float2(geA.y, geB.y), npy2);
-        float2 m1 = mul2_rn(dy2, make_float2(coA.z, coB.z));
-        const float2 m2 = mul2_rn(dx2, make_float2(coA.x, coB.x));
-        m1 = mul2_rn(dy2, m1);
-        const float2 sq = fma2_rn(dx2, m2, m1);
-        float2 m3 = mul2_rn(dx2, make_float2(coA.y, coB.y));
-        m3 = mul2_rn(dy2, m3);
-        const float2 npow = fma2_rn(sq, make_float2(0.5f, 0.5f), m3);  // = -power
+        const float2 npow = pair_npow(geA, geB, coA, coB, npx2, npy2);
         // order-dependent part (scalar): transmittance and the colour behind each record
 #pragma unroll
         for (int q = 0; q < 2; ++q) {

@@ -8,14 +8,13 @@
 //   feature_grad_finish_kernel  dL/dfeatures from the accumulators of every frame, which it re-zeroes
 //
 // One CTA per (tile, group of FG = 4 channels, frame): grid (T, ceil(C / 4), F).  Each CTA walks its tile's records
-// front to back in batches of RB, gathering the group's four feature values of each record from f[id] (a float4
-// per record in shared memory), so no workspace depends on the record capacity.  Both kernels repeat the
-// forward's blend operation for operation (same alpha, 1/255 skip, T recurrence and stop at n_contrib), so the
-// transmittance they see is the forward's bit for bit.
+// with the side passes' side_walk (raster_walk.cuh), so the transmittance it sees is the forward's bit for bit,
+// gathering the group's four feature values of each record from f[id] (a float4 per record in shared memory), so
+// no workspace depends on the record capacity.
 #include "../../include/dgmesh_b200.h"
 #include "common.cuh"
 #include "raster_kernels.h"
-#include "raster_bwd_blend.cuh"
+#include "raster_walk.cuh"
 
 namespace dgm {
 
@@ -40,17 +39,6 @@ __device__ __forceinline__ void load_feature_batch(const BinWS& b, uint32_t firs
   }
 }
 
-// max over the CTA of n_contrib (positions past it cannot contribute to any of its pixels)
-__device__ __forceinline__ int block_max_contrib(int v, int* s_maxc, uint32_t tid) {
-  if (tid == 0) *s_maxc = 0;
-  __syncthreads();
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
-  if ((tid & 31) == 0) atomicMax(s_maxc, v);
-  __syncthreads();
-  return *s_maxc;
-}
-
 }  // namespace
 
 // features [P,C] (per frame: frame f at features + f P C); out [F,C,H,W].  Frame f's workspaces at
@@ -65,83 +53,34 @@ __global__ void __launch_bounds__(256, 4) feature_fwd_kernel(int W, int H, int P
   __shared__ int s_maxc;
 
   const int f = blockIdx.z, c0 = blockIdx.y * FG;
-  const unsigned gx = (W + TILE_X - 1) / TILE_X, gy = (H + TILE_Y - 1) / TILE_Y;
+  SideTile t(W, H, f, img_ws, img_stride, bin_ws, bin_stride, R_cap);
+  t.find_stops(&s_maxc, [] {});
   const size_t npix = (size_t)W * H;
-  const ImgWS im = ImgWS::from(const_cast<char*>(img_ws) + f * img_stride, npix, (size_t)gx * gy);
-  const BinWS b = BinWS::from(const_cast<char*>(bin_ws) + f * bin_stride, (size_t)R_cap);
   const float* feats = features + (per_frame ? (size_t)f * P * C : 0);
 
-  const unsigned tile = im.tile_order[blockIdx.x];
-  const unsigned tx = tile % gx, ty = tile / gx;
-  const unsigned tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int wx0 = tx * TILE_X + (wid & 1) * 8, wy0 = ty * TILE_Y + (wid >> 1) * 4;
-  const int px = wx0 + (lane & 7), py = wy0 + (lane >> 3);
-  const bool inside = px < W && py < H;
-  const uint32_t pix_id = W * py + px;
-  const float bx0 = (float)wx0, bx1 = (float)(wx0 + 7), by0 = (float)wy0, by1 = (float)(wy0 + 3);
-  const float2 npx2 = make_float2(-(float)px, -(float)px), npy2 = make_float2(-(float)py, -(float)py);
-
-  const uint2 range = im.ranges[tile];
-  const int total = range.y - range.x;
-  const int last = inside ? (int)im.n_contrib[pix_id] : 0;
-  int wmax = last;
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
-  const int maxc = min(block_max_contrib(last, &s_maxc, tid), total);
-
   float T = 1.0f, F0 = 0.f, F1 = 0.f, F2 = 0.f, F3 = 0.f;
-  for (int base = 0; base < maxc; base += RB) {
-    const int cnt = min(RB, maxc - base);
-    __syncthreads();  // the previous batch is no longer read
-    load_feature_batch(b, range.x + base, cnt, feats, C, c0, s_geo, s_con, s_f, tid);
-    __syncthreads();
-    if (base >= wmax) continue;  // (uniform per warp) nothing left for this warp's pixels
-#pragma unroll 1
-    for (int k = 0; k < RB / 32; ++k) {
-      const int r = k * 32 + lane;
-      const bool kp = r < cnt && base + r < wmax && cull_keep(s_geo[r], s_con[r], bx0, bx1, by0, by1);
-      unsigned mask = __ballot_sync(0xffffffffu, kp);
-      while (mask) {
-        const int bA = __ffs(mask) - 1;
-        mask &= mask - 1;
-        const bool two = mask != 0;
-        const int bB = two ? __ffs(mask) - 1 : bA;
-        mask &= mask - 1;
-        const int jA = k * 32 + bA, jB = k * 32 + bB;
-        const float4 geA = s_geo[jA], geB = s_geo[jB];
-        const float4 coA = s_con[jA], coB = s_con[jB];
-        // the forward's quadratic form, operation for operation (raster_fwd.cu, render_fwd_kernel)
-        const float2 dx = add2_rn(make_float2(geA.x, geB.x), npx2);
-        const float2 dy = add2_rn(make_float2(geA.y, geB.y), npy2);
-        float2 m1 = mul2_rn(dy, make_float2(coA.z, coB.z));
-        const float2 m2 = mul2_rn(dx, make_float2(coA.x, coB.x));
-        m1 = mul2_rn(dy, m1);
-        const float2 sq = fma2_rn(dx, m2, m1);
-        float2 m3 = mul2_rn(dx, make_float2(coA.y, coB.y));
-        m3 = mul2_rn(dy, m3);
-        const float2 npow = fma2_rn(sq, make_float2(0.5f, 0.5f), m3);
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          const float np = q ? npow.y : npow.x;
-          const float opac = q ? coB.w : coA.w;
-          const int j = q ? jB : jA;
-          if ((q == 0 || two) && base + j < last && !(np < 0.0f)) {
-            const float alpha = fminf(0.99f, __fmul_rn(opac, expf(-np)));
-            if (!(alpha < 1.0f / 255.0f)) {
-              const float4 fv = s_f[j];
-              F0 = __fmaf_rn(T, __fmul_rn(alpha, fv.x), F0);
-              F1 = __fmaf_rn(T, __fmul_rn(alpha, fv.y), F1);
-              F2 = __fmaf_rn(T, __fmul_rn(alpha, fv.z), F2);
-              F3 = __fmaf_rn(T, __fmul_rn(alpha, fv.w), F3);
-              T = __fmul_rn(T, __fadd_rn(1.0f, -alpha));
-            }
+  // (the record callable's capture order sets nvcc's register assignment of the sums: compare SASS when changing it)
+  side_walk(
+      t, s_geo, s_con,
+      [&](int base, int cnt) {
+        load_feature_batch(t.b, t.range.x + base, cnt, feats, C, c0, s_geo, s_con, s_f, t.tid);
+      },
+      [&F3, &F2, &F1, &F0, &T](int, int j, float opac, float np, bool pre) {
+        if (pre) {
+          const float alpha = fminf(0.99f, __fmul_rn(opac, expf(-np)));
+          if (!(alpha < 1.0f / 255.0f)) {
+            const float4 fv = s_f[j];
+            F0 = __fmaf_rn(T, __fmul_rn(alpha, fv.x), F0);
+            F1 = __fmaf_rn(T, __fmul_rn(alpha, fv.y), F1);
+            F2 = __fmaf_rn(T, __fmul_rn(alpha, fv.z), F2);
+            F3 = __fmaf_rn(T, __fmul_rn(alpha, fv.w), F3);
+            T = __fmul_rn(T, __fadd_rn(1.0f, -alpha));
           }
         }
-      }
-    }
-  }
-  if (inside) {
-    float* o = out + ((size_t)f * C + c0) * npix + pix_id;
+      },
+      [](int) {});
+  if (t.inside) {
+    float* o = out + ((size_t)f * C + c0) * npix + t.pix_id;
     const float v[FG] = {F0, F1, F2, F3};
 #pragma unroll
     for (int k = 0; k < FG; ++k)
@@ -175,151 +114,103 @@ __global__ void __launch_bounds__(256, 2) feature_bwd_kernel(int W, int H, int P
 
   const int f = blockIdx.z, c0 = blockIdx.y * FG;
   const int Cp = (C + FG - 1) / FG * FG;
-  const unsigned gx = (W + TILE_X - 1) / TILE_X, gy = (H + TILE_Y - 1) / TILE_Y;
+  SideTile t(W, H, f, img_ws, img_stride, bin_ws, bin_stride, R_cap);
   const size_t npix = (size_t)W * H;
-  const ImgWS im = ImgWS::from(const_cast<char*>(img_ws) + f * img_stride, npix, (size_t)gx * gy);
-  const BinWS b = BinWS::from(const_cast<char*>(bin_ws) + f * bin_stride, (size_t)R_cap);
   float4* const grad_acc = GeomWS::from(geom_ws + f * geom_stride, P).grad_acc;
   float* const facc = reinterpret_cast<float*>(feat_ws + f * ws_stride);
   const float* feats = features + (per_frame ? (size_t)f * P * C : 0);
-
-  const unsigned tile = im.tile_order[blockIdx.x];
-  const unsigned tx = tile % gx, ty = tile / gx;
-  const unsigned tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int wx0 = tx * TILE_X + (wid & 1) * 8, wy0 = ty * TILE_Y + (wid >> 1) * 4;
-  const int px = wx0 + (lane & 7), py = wy0 + (lane >> 3);
-  const bool inside = px < W && py < H;
-  const uint32_t pix_id = W * py + px;
-  const float bx0 = (float)wx0, bx1 = (float)(wx0 + 7), by0 = (float)wy0, by1 = (float)(wy0 + 3);
-  const float cx = wx0 + 3.5f, cy = wy0 + 1.5f;  // centre of the warp's block
-  const float2 npx2 = make_float2(-(float)px, -(float)px), npy2 = make_float2(-(float)py, -(float)py);
-
-  const uint2 range = im.ranges[tile];
-  const int total = range.y - range.x;
-  const int last = inside ? (int)im.n_contrib[pix_id] : 0;
-  int wmax = last;
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
-  for (int i = tid; i < RB * ACC_STRIDE; i += 256) s_acc[i] = 0.f;
-  const int maxc = min(block_max_contrib(last, &s_maxc, tid), total);
-  if (maxc == 0) return;  // uniform per CTA
+  const float cx = t.wx0 + 3.5f, cy = t.wy0 + 1.5f;  // centre of the warp's block
+  t.find_stops(&s_maxc, [&] {
+    for (int i = t.tid; i < RB * ACC_STRIDE; i += 256) s_acc[i] = 0.f;
+  });
+  if (t.maxc == 0) return;  // uniform per CTA
 
   // the group's upstream gradient (the dL/dpixel rows of the contraction) and map values of this pixel
   float g[FG], Fm[FG], Pf[FG];
 #pragma unroll
   for (int k = 0; k < FG; ++k) {
-    const bool ok = inside && c0 + k < C;
-    const size_t o = ((size_t)f * C + c0 + k) * npix + pix_id;
+    const bool ok = t.inside && c0 + k < C;
+    const size_t o = ((size_t)f * C + c0 + k) * npix + t.pix_id;
     g[k] = ok ? dL_dfmap[o] : 0.0f;
     Fm[k] = ok ? fmap[o] : 0.0f;
     Pf[k] = 0.0f;
-    s_dlp[wid][k][lane] = g[k];
+    s_dlp[t.wid][k][t.lane] = g[k];
   }
-  float* const stage = s_stage + wid * (CHUNK * SLOT_F);
+  float* const stage = s_stage + t.wid * (CHUNK * SLOT_F);
   int nslot = 0, rec = 0;  // staged records; the record of slot lane & 15
   float T = 1.0f;
 
-  for (int base = 0; base < maxc; base += RB) {
-    const int cnt = min(RB, maxc - base);
-    __syncthreads();  // the previous batch is flushed
-    load_feature_batch(b, range.x + base, cnt, feats, C, c0, s_geo, s_con, s_f, tid);
-    if ((int)tid < cnt) s_id[tid] = __float_as_uint(b.inst_attr[2 * ((size_t)range.x + base + tid) + 1].w);
-    __syncthreads();
-    if (base < wmax) {  // (uniform per warp)
-#pragma unroll 1
-      for (int k = 0; k < RB / 32; ++k) {
-        const int r = k * 32 + lane;
-        const bool kp = r < cnt && base + r < wmax && cull_keep(s_geo[r], s_con[r], bx0, bx1, by0, by1);
-        unsigned mask = __ballot_sync(0xffffffffu, kp);
-        while (mask) {
-          const int bA = __ffs(mask) - 1;
-          mask &= mask - 1;
-          const bool two = mask != 0;
-          const int bB = two ? __ffs(mask) - 1 : bA;
-          mask &= mask - 1;
-          const int jA = k * 32 + bA, jB = k * 32 + bB;
-          const float4 geA = s_geo[jA], geB = s_geo[jB];
-          const float4 coA = s_con[jA], coB = s_con[jB];
-          const float2 dx = add2_rn(make_float2(geA.x, geB.x), npx2);
-          const float2 dy = add2_rn(make_float2(geA.y, geB.y), npy2);
-          float2 m1 = mul2_rn(dy, make_float2(coA.z, coB.z));
-          const float2 m2 = mul2_rn(dx, make_float2(coA.x, coB.x));
-          m1 = mul2_rn(dy, m1);
-          const float2 sq = fma2_rn(dx, m2, m1);
-          float2 m3 = mul2_rn(dx, make_float2(coA.y, coB.y));
-          m3 = mul2_rn(dy, m3);
-          const float2 npow = fma2_rn(sq, make_float2(0.5f, 0.5f), m3);
+  side_walk(
+      t, s_geo, s_con,
+      [&](int base, int cnt) {
+        load_feature_batch(t.b, t.range.x + base, cnt, feats, C, c0, s_geo, s_con, s_f, t.tid);
+        if ((int)t.tid < cnt)
+          s_id[t.tid] = __float_as_uint(t.b.inst_attr[2 * ((size_t)t.range.x + base + t.tid) + 1].w);
+      },
+      [&](int q, int j, float opac, float np, bool pre) {
+        const float G = expf(-np);
+        const float alpha = fminf(0.99f, __fmul_rn(opac, G));
+        const bool act = pre && !(alpha < 1.0f / 255.0f);
+        const float4 fv = s_f[j];
+        const float fa[FG] = {fv.x, fv.y, fv.z, fv.w};
+        const float r1 = __fdividef(1.0f, 1.0f - alpha);
+        float dLa = 0.0f;
 #pragma unroll
-          for (int q = 0; q < 2; ++q) {
-            const float np = q ? npow.y : npow.x;
-            const float opac = q ? coB.w : coA.w;
-            const int j = q ? jB : jA;
-            const bool pre = (q == 0 || two) && base + j < last && !(np < 0.0f);
-            const float G = expf(-np);
-            const float alpha = fminf(0.99f, __fmul_rn(opac, G));
-            const bool act = pre && !(alpha < 1.0f / 255.0f);
-            const float4 fv = s_f[j];
-            const float fa[FG] = {fv.x, fv.y, fv.z, fv.w};
-            const float r1 = __fdividef(1.0f, 1.0f - alpha);
-            float dLa = 0.0f;
+        for (int c = 0; c < FG; ++c) {
+          const float pn = __fmaf_rn(T, __fmul_rn(alpha, fa[c]), Pf[c]);
+          Pf[c] = act ? pn : Pf[c];
+          dLa = fmaf(g[c], fmaf(T, fa[c], -(Fm[c] - Pf[c]) * r1), dLa);
+        }
+        const float w = act ? (G * opac) * dLa : 0.0f;
+        const float aT = act ? alpha * T : 0.0f;
+        T = act ? __fmul_rn(T, __fadd_rn(1.0f, -alpha)) : T;
+        if (__any_sync(0xffffffffu, act)) {
+          stage[nslot * SLOT_F + t.lane] = w;
+          stage[nslot * SLOT_F + 32 + t.lane] = aT;
+          if ((int)(t.lane & 15) == nslot) rec = j;
+          ++nslot;
+        }
+        if (q == 1 && nslot > CHUNK - 2) {  // the pair is staged and there is no room for another
+          __syncwarp();
+          contract_chunk<true>(stage, &s_dlp[t.wid][0][0], nslot, rec, t.lane, s_geo, cx, cy, s_acc);
+          __syncwarp();
+          nslot = 0;
+        }
+      },
+      [&](int cnt) {
+        if (nslot > 0) {  // the batch's records must be in s_acc before the flush
+          __syncwarp();
+          contract_chunk<true>(stage, &s_dlp[t.wid][0][0], nslot, rec, t.lane, s_geo, cx, cy, s_acc);
+          __syncwarp();
+          nslot = 0;
+        }
+        __syncthreads();
+        // ---- flush this batch: the moments as the blend backward turns them into gradients, and the feature sums
+        if ((int)t.tid < cnt) {
+          float* acc = &s_acc[t.tid * ACC_STRIDE];
+          float a[ACC_STRIDE];
+          bool nz = false;
 #pragma unroll
-            for (int c = 0; c < FG; ++c) {
-              const float pn = __fmaf_rn(T, __fmul_rn(alpha, fa[c]), Pf[c]);
-              Pf[c] = act ? pn : Pf[c];
-              dLa = fmaf(g[c], fmaf(T, fa[c], -(Fm[c] - Pf[c]) * r1), dLa);
-            }
-            const float w = act ? (G * opac) * dLa : 0.0f;
-            const float aT = act ? alpha * T : 0.0f;
-            T = act ? __fmul_rn(T, __fadd_rn(1.0f, -alpha)) : T;
-            if (__any_sync(0xffffffffu, act)) {
-              stage[nslot * SLOT_F + lane] = w;
-              stage[nslot * SLOT_F + 32 + lane] = aT;
-              if ((int)(lane & 15) == nslot) rec = j;
-              ++nslot;
-            }
+          for (int q = 0; q < ACC_STRIDE; ++q) {
+            a[q] = acc[q];
+            nz |= (a[q] != 0.f);
+            acc[q] = 0.f;
           }
-          if (nslot > CHUNK - 2) {  // no room for another pair
-            __syncwarp();
-            contract_chunk<true>(stage, &s_dlp[wid][0][0], nslot, rec, lane, s_geo, cx, cy, s_acc);
-            __syncwarp();
-            nslot = 0;
+          if (nz) {
+            const float ddelx_dx = 0.5 * W;
+            const float ddely_dy = 0.5 * H;
+            const float4 con_o = s_con[t.tid];
+            const uint32_t id = s_id[t.tid];
+            const float g_mx = -ddelx_dx * (con_o.x * a[1] + con_o.y * a[2]);
+            const float g_my = -ddely_dy * (con_o.z * a[2] + con_o.y * a[1]);
+            const float g_op = (con_o.w != 0.0f) ? a[0] / con_o.w : 0.0f;
+            float* dst = reinterpret_cast<float*>(grad_acc + 3 * (size_t)id);
+            red_add_v4(dst, g_mx, g_my, -0.5f * a[3], -0.5f * a[4]);
+            red_add_v2(dst + 4, -0.5f * a[5], g_op);
+            red_add_v4(facc + (size_t)id * Cp + c0, a[6], a[7], a[8], a[9]);
           }
         }
-      }
-      if (nslot > 0) {  // the batch's records must be in s_acc before the flush
-        __syncwarp();
-        contract_chunk<true>(stage, &s_dlp[wid][0][0], nslot, rec, lane, s_geo, cx, cy, s_acc);
-        __syncwarp();
-        nslot = 0;
-      }
-    }
-    __syncthreads();
-    // ---- flush this batch: the moments as the blend backward turns them into gradients, and the feature sums
-    if ((int)tid < cnt) {
-      float* acc = &s_acc[tid * ACC_STRIDE];
-      float a[ACC_STRIDE];
-      bool nz = false;
-#pragma unroll
-      for (int q = 0; q < ACC_STRIDE; ++q) {
-        a[q] = acc[q];
-        nz |= (a[q] != 0.f);
-        acc[q] = 0.f;
-      }
-      if (nz) {
-        const float ddelx_dx = 0.5 * W;
-        const float ddely_dy = 0.5 * H;
-        const float4 con_o = s_con[tid];
-        const uint32_t id = s_id[tid];
-        const float g_mx = -ddelx_dx * (con_o.x * a[1] + con_o.y * a[2]);
-        const float g_my = -ddely_dy * (con_o.z * a[2] + con_o.y * a[1]);
-        const float g_op = (con_o.w != 0.0f) ? a[0] / con_o.w : 0.0f;
-        float* dst = reinterpret_cast<float*>(grad_acc + 3 * (size_t)id);
-        red_add_v4(dst, g_mx, g_my, -0.5f * a[3], -0.5f * a[4]);
-        red_add_v2(dst + 4, -0.5f * a[5], g_op);
-        red_add_v4(facc + (size_t)id * Cp + c0, a[6], a[7], a[8], a[9]);
-      }
-    }
-  }
+      });
 }
 
 // dL/dfeatures from the feature accumulators of F frames, one thread per (Gaussian, padded channel): per_frame,

@@ -734,11 +734,8 @@ __global__ void __launch_bounds__(256, AUX ? 4 : 5) render_fwd_kernel(const uint
     if (lane == 0) atomicAdd(&g_dbg_pairs[2], (unsigned long long)nb);
 #endif
     // ---- blend the survivors front to back, two records per iteration: the quadratic
-    // forms of both are evaluated side by side (add2_rn / mul2_rn / fma2_rn), the
-    // order-dependent transmittance update stays scalar.  The operation
-    // sequence (which product is fused into which FMA) is the one nvcc emits for the
-    // reference's renderCUDA (forward.cu:330-352),
-    // written with explicit-rounding intrinsics so it cannot be re-associated.
+    // forms of both are evaluated side by side (pair_npow), the order-dependent
+    // transmittance update stays scalar.
 #pragma unroll
     for (int k = 0; k < RB / 32; ++k) {
       unsigned mask = keep[k];
@@ -753,15 +750,7 @@ __global__ void __launch_bounds__(256, AUX ? 4 : 5) render_fwd_kernel(const uint
         const int jA = k * 32 + bA, jB = k * 32 + bB;
         const float4 geA = s_geo[st][jA], geB = s_geo[st][jB];
         const float4 coA = s_attr[st][2 * jA], coB = s_attr[st][2 * jB];
-        const float2 dx = add2_rn(make_float2(geA.x, geB.x), npx2);
-        const float2 dy = add2_rn(make_float2(geA.y, geB.y), npy2);
-        float2 m1 = mul2_rn(dy, make_float2(coA.z, coB.z));
-        const float2 m2 = mul2_rn(dx, make_float2(coA.x, coB.x));
-        m1 = mul2_rn(dy, m1);
-        const float2 sq = fma2_rn(dx, m2, m1);
-        float2 m3 = mul2_rn(dx, make_float2(coA.y, coB.y));
-        m3 = mul2_rn(dy, m3);
-        const float2 npow = fma2_rn(sq, make_float2(0.5f, 0.5f), m3);  // = -power (exactly)
+        const float2 npow = pair_npow(geA, geB, coA, coB, npx2, npy2);
 #ifdef DGM_COUNT_PAIRS
         const uint32_t lc_before = last_contributor;
 #endif

@@ -32,6 +32,23 @@ __device__ __forceinline__ float2 fma2_rn(float2 a, float2 b, float2 c) {
   return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
+// The quadratic form of two blend records A, B (geo: mean in .xy; con: conic in .xyz) at the pixel (-npx, -npy),
+// side by side.  The operation sequence (which product is fused into which FMA) is the one nvcc emits for the
+// reference's renderCUDA (forward.cu:330-352), written with explicit-rounding intrinsics so it cannot be
+// re-associated: every blend kernel and side pass sees the same value, = -power (exactly).
+__device__ __forceinline__ float2 pair_npow(float4 geA, float4 geB, float4 coA, float4 coB, float2 npx2,
+                                            float2 npy2) {
+  const float2 dx = add2_rn(make_float2(geA.x, geB.x), npx2);
+  const float2 dy = add2_rn(make_float2(geA.y, geB.y), npy2);
+  float2 m1 = mul2_rn(dy, make_float2(coA.z, coB.z));
+  const float2 m2 = mul2_rn(dx, make_float2(coA.x, coB.x));
+  m1 = mul2_rn(dy, m1);
+  const float2 sq = fma2_rn(dx, m2, m1);
+  float2 m3 = mul2_rn(dx, make_float2(coA.y, coB.y));
+  m3 = mul2_rn(dy, m3);
+  return fma2_rn(sq, make_float2(0.5f, 0.5f), m3);
+}
+
 struct Mat3 {  // column-major like glm: c[col][row]
   float c[3][3];
 };

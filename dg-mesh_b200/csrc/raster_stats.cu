@@ -5,31 +5,14 @@
 //   blend_stats_kernel  sum_i = sum_p e_p alpha_ip T_ip and max_i = max(0, max_p e_p alpha_ip T_ip) over the colour
 //                       image's own blend, e_p an optional per-pixel weight (1 when absent)
 //
-// One CTA per (tile, frame): grid (T, F).  The walk is feature_fwd_kernel's (raster_feat.cu): batches of RB
-// records in shared memory, cull_keep per warp, the forward's quadratic form operation for operation, the 1/255
-// skip and the stop at n_contrib, so T is the forward's bit for bit.  It is kept as a copy rather than a device
-// helper shared with feature_fwd_kernel so that the feature kernels' code stays exactly as it is.
+// One CTA per (tile, frame): grid (T, F).  The walk is the side passes' side_walk (raster_walk.cuh), so T is the
+// forward's bit for bit.
 #include "../../include/dgmesh_b200.h"
 #include "common.cuh"
 #include "raster_kernels.h"
-#include "raster_bwd_blend.cuh"
+#include "raster_walk.cuh"
 
 namespace dgm {
-
-namespace {
-
-// max over the CTA of n_contrib (positions past it cannot contribute to any of its pixels)
-__device__ __forceinline__ int stats_block_max_contrib(int v, int* s_maxc, uint32_t tid) {
-  if (tid == 0) *s_maxc = 0;
-  __syncthreads();
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
-  if ((tid & 31) == 0) atomicMax(s_maxc, v);
-  __syncthreads();
-  return *s_maxc;
-}
-
-}  // namespace
 
 // Each blended (pixel, record) pair gives v = e_p alpha T.  Per record the warp forms the total of v over its 32
 // pixels (a fixed butterfly) and the maximum (__reduce_max_sync on the bits: v is clamped to >= 0 first, and the
@@ -51,115 +34,65 @@ __global__ void __launch_bounds__(256, 4) blend_stats_kernel(int W, int H, int P
   __shared__ int s_maxc;
 
   const int f = blockIdx.y;
-  const unsigned gx = (W + TILE_X - 1) / TILE_X, gy = (H + TILE_Y - 1) / TILE_Y;
-  const size_t npix = (size_t)W * H;
-  const ImgWS im = ImgWS::from(const_cast<char*>(img_ws) + f * img_stride, npix, (size_t)gx * gy);
-  const BinWS b = BinWS::from(const_cast<char*>(bin_ws) + f * bin_stride, (size_t)R_cap);
-
-  const unsigned tile = im.tile_order[blockIdx.x];
-  const unsigned tx = tile % gx, ty = tile / gx;
-  const unsigned tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int wx0 = tx * TILE_X + (wid & 1) * 8, wy0 = ty * TILE_Y + (wid >> 1) * 4;
-  const int px = wx0 + (lane & 7), py = wy0 + (lane >> 3);
-  const bool inside = px < W && py < H;
-  const uint32_t pix_id = W * py + px;
-  const float bx0 = (float)wx0, bx1 = (float)(wx0 + 7), by0 = (float)wy0, by1 = (float)(wy0 + 3);
-  const float2 npx2 = make_float2(-(float)px, -(float)px), npy2 = make_float2(-(float)py, -(float)py);
-  const float e = (weights && inside) ? weights[f * w_stride + pix_id] : 1.0f;
-
-  const uint2 range = im.ranges[tile];
-  const int total = range.y - range.x;
-  const int last = inside ? (int)im.n_contrib[pix_id] : 0;
-  int wmax = last;
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
-  for (int i = tid; i < 8 * RB; i += 256) {  // the flush re-zeroes the slots it reads
-    (&s_sum[0][0])[i] = 0.0f;
-    (&s_max[0][0])[i] = 0u;
-  }
-  const int maxc = min(stats_block_max_contrib(last, &s_maxc, tid), total);
-  float* const my_sum = s_sum[wid];
-  unsigned* const my_max = s_max[wid];
+  SideTile t(W, H, f, img_ws, img_stride, bin_ws, bin_stride, R_cap);
+  const float e = (weights && t.inside) ? weights[f * w_stride + t.pix_id] : 1.0f;
+  t.find_stops(&s_maxc, [&] {
+    for (int i = t.tid; i < 8 * RB; i += 256) {  // the flush re-zeroes the slots it reads
+      (&s_sum[0][0])[i] = 0.0f;
+      (&s_max[0][0])[i] = 0u;
+    }
+  });
+  float* const my_sum = s_sum[t.wid];
+  unsigned* const my_max = s_max[t.wid];
 
   float T = 1.0f;
-  for (int base = 0; base < maxc; base += RB) {
-    const int cnt = min(RB, maxc - base);
-    __syncthreads();  // the previous batch is flushed
-    if ((int)tid < cnt) {
-      const size_t r = (size_t)range.x + base + tid;
-      s_geo[tid] = b.inst_geo[r];
-      s_con[tid] = b.inst_attr[2 * r];
-      s_id[tid] = __float_as_uint(b.inst_attr[2 * r + 1].w);
-    }
-    __syncthreads();
-    if (base < wmax) {  // (uniform per warp) something left for this warp's pixels
-#pragma unroll 1
-      for (int k = 0; k < RB / 32; ++k) {
-        const int r = k * 32 + lane;
-        const bool kp = r < cnt && base + r < wmax && cull_keep(s_geo[r], s_con[r], bx0, bx1, by0, by1);
-        unsigned mask = __ballot_sync(0xffffffffu, kp);
-        while (mask) {
-          const int bA = __ffs(mask) - 1;
-          mask &= mask - 1;
-          const bool two = mask != 0;
-          const int bB = two ? __ffs(mask) - 1 : bA;
-          mask &= mask - 1;
-          const int jA = k * 32 + bA, jB = k * 32 + bB;
-          const float4 geA = s_geo[jA], geB = s_geo[jB];
-          const float4 coA = s_con[jA], coB = s_con[jB];
-          // the forward's quadratic form, operation for operation (raster_fwd.cu, render_fwd_kernel)
-          const float2 dx = add2_rn(make_float2(geA.x, geB.x), npx2);
-          const float2 dy = add2_rn(make_float2(geA.y, geB.y), npy2);
-          float2 m1 = mul2_rn(dy, make_float2(coA.z, coB.z));
-          const float2 m2 = mul2_rn(dx, make_float2(coA.x, coB.x));
-          m1 = mul2_rn(dy, m1);
-          const float2 sq = fma2_rn(dx, m2, m1);
-          float2 m3 = mul2_rn(dx, make_float2(coA.y, coB.y));
-          m3 = mul2_rn(dy, m3);
-          const float2 npow = fma2_rn(sq, make_float2(0.5f, 0.5f), m3);
-#pragma unroll
-          for (int q = 0; q < 2; ++q) {
-            const float np = q ? npow.y : npow.x;
-            const float opac = q ? coB.w : coA.w;
-            const int j = q ? jB : jA;
-            float v = 0.0f;
-            if ((q == 0 || two) && base + j < last && !(np < 0.0f)) {
-              const float alpha = fminf(0.99f, __fmul_rn(opac, expf(-np)));
-              if (!(alpha < 1.0f / 255.0f)) {
-                v = __fmul_rn(e, __fmul_rn(alpha, T));
-                T = __fmul_rn(T, __fadd_rn(1.0f, -alpha));
-              }
-            }
-            const unsigned vb = v > 0.0f ? __float_as_uint(v) : 0u;
-            // (uniform per warp) a record no pixel of the warp blends leaves its slots at zero
-            if (__ballot_sync(0xffffffffu, v != 0.0f) != 0u) {
-              float s = v;
-#pragma unroll
-              for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-              const unsigned m = __reduce_max_sync(0xffffffffu, vb);
-              if (lane == 0) my_sum[j] = s, my_max[j] = m;
-            }
+  side_walk(
+      t, s_geo, s_con,
+      [&](int base, int cnt) {
+        if ((int)t.tid < cnt) {
+          const size_t r = (size_t)t.range.x + base + t.tid;
+          s_geo[t.tid] = t.b.inst_geo[r];
+          s_con[t.tid] = t.b.inst_attr[2 * r];
+          s_id[t.tid] = __float_as_uint(t.b.inst_attr[2 * r + 1].w);
+        }
+      },
+      [&](int, int j, float opac, float np, bool pre) {
+        float v = 0.0f;
+        if (pre) {
+          const float alpha = fminf(0.99f, __fmul_rn(opac, expf(-np)));
+          if (!(alpha < 1.0f / 255.0f)) {
+            v = __fmul_rn(e, __fmul_rn(alpha, T));
+            T = __fmul_rn(T, __fadd_rn(1.0f, -alpha));
           }
         }
-      }
-    }
-    __syncthreads();
-    // ---- flush this batch: one total per record, the 8 warps in warp order
-    if ((int)tid < cnt) {
-      float s = 0.0f;
-      unsigned m = 0u;
+        const unsigned vb = v > 0.0f ? __float_as_uint(v) : 0u;
+        // (uniform per warp) a record no pixel of the warp blends leaves its slots at zero
+        if (__ballot_sync(0xffffffffu, v != 0.0f) != 0u) {
+          float s = v;
 #pragma unroll
-      for (int w = 0; w < 8; ++w) {
-        s += s_sum[w][tid];
-        m = max(m, s_max[w][tid]);
-        s_sum[w][tid] = 0.0f;
-        s_max[w][tid] = 0u;
-      }
-      const size_t id = (size_t)f * P + s_id[tid];
-      if (s != 0.0f) atomicAdd(out_sum + id, s);
-      if (m != 0u) atomicMax(out_max + id, m);
-    }
-  }
+          for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+          const unsigned m = __reduce_max_sync(0xffffffffu, vb);
+          if (t.lane == 0) my_sum[j] = s, my_max[j] = m;
+        }
+      },
+      [&](int cnt) {
+        __syncthreads();
+        // ---- flush this batch: one total per record, the 8 warps in warp order
+        if ((int)t.tid < cnt) {
+          float s = 0.0f;
+          unsigned m = 0u;
+#pragma unroll
+          for (int w = 0; w < 8; ++w) {
+            s += s_sum[w][t.tid];
+            m = max(m, s_max[w][t.tid]);
+            s_sum[w][t.tid] = 0.0f;
+            s_max[w][t.tid] = 0u;
+          }
+          const size_t id = (size_t)f * P + s_id[t.tid];
+          if (s != 0.0f) atomicAdd(out_sum + id, s);
+          if (m != 0u) atomicMax(out_max + id, m);
+        }
+      });
 }
 
 cudaError_t launch_blend_stats(const StatsArgs& a, cudaStream_t s) {
