@@ -932,23 +932,43 @@ int dgr_feature_workspace_size(int P, int C, int F, size_t* bytes) {
 }
 
 namespace {
-// the arguments shared by dgr_features_fwd / _bwd: DGM_OK, or the error to return (nothing is launched)
-int feature_args(const char* who, int F, int P, int C, int W, int H, const float* features, void* geom_ws,
-                 size_t geom_stride, void* binning_ws, size_t binning_stride, int64_t R_cap, void* img_ws,
-                 size_t img_stride, void* feat_ws, size_t feat_ws_bytes) {
+// The workspaces of F frames an earlier forward wrote, as a side-pass entry point (who) takes them: DGM_OK with ws
+// filled in, or the error to return (nothing is launched).  The pass's own pointers are checked with them (own_ptrs:
+// none is NULL).  max_F: PB_MAX_FRAMES for the passes whose workspaces are sized per frame, 65535 (grid.y) for
+// blend statistics, which reads no geometry workspace (geom false: geom_ws and geom_stride are not checked).
+int forward_ws_args(const char* who, int max_F, bool geom, int F, int P, int W, int H, void* geom_ws,
+                    size_t geom_stride, void* binning_ws, size_t binning_stride, int64_t R_cap, void* img_ws,
+                    size_t img_stride, bool own_ptrs, dgm::ForwardWS& ws) {
   char msg[128];
-  if (C < 1 || C > 64) return snprintf(msg, sizeof(msg), "%s: need 1 <= C <= 64", who), bad(msg);
-  if (F < 1 || F > PB_MAX_FRAMES || P < 0 || W <= 0 || H <= 0 || R_cap < 0)
+  if (F < 1 || F > max_F || P < 0 || W <= 0 || H <= 0 || R_cap < 0)
     return snprintf(msg, sizeof(msg), "%s: bad size", who), bad(msg);
-  if (!features || !geom_ws || !binning_ws || !img_ws || !feat_ws)
+  if ((geom && !geom_ws) || !binning_ws || !img_ws || !own_ptrs)
     return snprintf(msg, sizeof(msg), "%s: null pointer", who), bad(msg);
   if (F > 1) {
     size_t gb, bb, ib;
     dgr_workspace_sizes(P, W, H, R_cap, &gb, &bb, &ib);
-    if (geom_stride < gb || binning_stride < bb || img_stride < ib || geom_stride % 128 || binning_stride % 128 ||
-        img_stride % 128)
+    if ((geom && (geom_stride < gb || geom_stride % 128)) || binning_stride < bb || img_stride < ib ||
+        binning_stride % 128 || img_stride % 128)
       return snprintf(msg, sizeof(msg), "%s: workspace stride too small or not a multiple of 128", who), bad(msg);
   }
+  ws.F = F, ws.P = P, ws.W = W, ws.H = H;
+  ws.geom_ws = geom_ws, ws.binning_ws = binning_ws, ws.img_ws = img_ws;
+  ws.geom_stride = F > 1 ? geom_stride : 0, ws.binning_stride = F > 1 ? binning_stride : 0;
+  ws.img_stride = F > 1 ? img_stride : 0;
+  ws.R_cap = R_cap;
+  return DGM_OK;
+}
+
+// the arguments shared by dgr_features_fwd / _bwd: DGM_OK, or the error to return (nothing is launched)
+int feature_args(const char* who, int F, int P, int C, int W, int H, const float* features, int per_frame,
+                 void* geom_ws, size_t geom_stride, void* binning_ws, size_t binning_stride, int64_t R_cap,
+                 void* img_ws, size_t img_stride, void* feat_ws, size_t feat_ws_bytes, dgm::FeatArgs& a) {
+  char msg[128];
+  if (C < 1 || C > 64) return snprintf(msg, sizeof(msg), "%s: need 1 <= C <= 64", who), bad(msg);
+  a = {};
+  const int rc = forward_ws_args(who, PB_MAX_FRAMES, true, F, P, W, H, geom_ws, geom_stride, binning_ws,
+                                 binning_stride, R_cap, img_ws, img_stride, features && feat_ws, a);
+  if (rc != DGM_OK) return rc;
   if (reinterpret_cast<uintptr_t>(feat_ws) % 16) return snprintf(msg, sizeof(msg), "%s: misaligned workspace", who), bad(msg);
   size_t need;
   dgr_feature_workspace_size(P, C, F, &need);
@@ -956,32 +976,19 @@ int feature_args(const char* who, int F, int P, int C, int W, int H, const float
     snprintf(g_last_error, sizeof(g_last_error), "%s: feature workspace too small", who);
     return DGM_E_WORKSPACE;
   }
+  a.C = C, a.features = features, a.per_frame = per_frame ? 1 : 0, a.feat_ws = feat_ws;
   return DGM_OK;
-}
-
-dgm::FeatArgs feature_call(int F, int P, int C, int W, int H, const float* features, int per_frame, void* geom_ws,
-                           size_t geom_stride, void* binning_ws, size_t binning_stride, int64_t R_cap, void* img_ws,
-                           size_t img_stride, void* feat_ws) {
-  dgm::FeatArgs a = {};
-  a.F = F, a.P = P, a.C = C, a.W = W, a.H = H;
-  a.features = features, a.per_frame = per_frame ? 1 : 0;
-  a.geom_ws = geom_ws, a.binning_ws = binning_ws, a.img_ws = img_ws;
-  a.geom_stride = F > 1 ? geom_stride : 0, a.binning_stride = F > 1 ? binning_stride : 0;
-  a.img_stride = F > 1 ? img_stride : 0;
-  a.R_cap = R_cap, a.feat_ws = feat_ws;
-  return a;
 }
 }  // namespace
 
 int dgr_features_fwd(int F, int P, int C, int W, int H, const float* features, int features_per_frame, void* geom_ws,
                      size_t geom_stride, void* binning_ws, size_t binning_stride, int64_t R_cap, void* img_ws,
                      size_t img_stride, float* out_map, void* feat_ws, size_t feat_ws_bytes, void* stream) {
-  const int rc = feature_args("dgr_features_fwd", F, P, C, W, H, features, geom_ws, geom_stride, binning_ws,
-                              binning_stride, R_cap, img_ws, img_stride, feat_ws, feat_ws_bytes);
+  dgm::FeatArgs a;
+  const int rc = feature_args("dgr_features_fwd", F, P, C, W, H, features, features_per_frame, geom_ws, geom_stride,
+                              binning_ws, binning_stride, R_cap, img_ws, img_stride, feat_ws, feat_ws_bytes, a);
   if (rc != DGM_OK) return rc;
   if (!out_map) return bad("dgr_features_fwd: null pointer");
-  dgm::FeatArgs a = feature_call(F, P, C, W, H, features, features_per_frame, geom_ws, geom_stride, binning_ws,
-                                 binning_stride, R_cap, img_ws, img_stride, feat_ws);
   a.out_map = out_map;
   return check(dgm::launch_features_fwd(a, (cudaStream_t)stream));
 }
@@ -990,12 +997,11 @@ int dgr_features_bwd(int F, int P, int C, int W, int H, const float* features, i
                      size_t geom_stride, void* binning_ws, size_t binning_stride, int64_t R_cap, void* img_ws,
                      size_t img_stride, const float* map, const float* dL_dmap, float* dL_dfeatures, void* feat_ws,
                      size_t feat_ws_bytes, void* stream) {
-  const int rc = feature_args("dgr_features_bwd", F, P, C, W, H, features, geom_ws, geom_stride, binning_ws,
-                              binning_stride, R_cap, img_ws, img_stride, feat_ws, feat_ws_bytes);
+  dgm::FeatArgs a;
+  const int rc = feature_args("dgr_features_bwd", F, P, C, W, H, features, features_per_frame, geom_ws, geom_stride,
+                              binning_ws, binning_stride, R_cap, img_ws, img_stride, feat_ws, feat_ws_bytes, a);
   if (rc != DGM_OK) return rc;
   if (!map || !dL_dmap) return bad("dgr_features_bwd: null pointer");
-  dgm::FeatArgs a = feature_call(F, P, C, W, H, features, features_per_frame, geom_ws, geom_stride, binning_ws,
-                                 binning_stride, R_cap, img_ws, img_stride, feat_ws);
   a.map = map, a.dL_dmap = dL_dmap, a.dL_dfeatures = dL_dfeatures;
   return check(dgm::launch_features_bwd(a, (cudaStream_t)stream));
 }
@@ -1025,17 +1031,10 @@ int planar_args(const char* who, int F, int P, int W, int H, const float* planes
                 void* binning_ws, size_t binning_stride, int64_t R_cap, void* img_ws, size_t img_stride,
                 void* planar_ws, size_t planar_ws_bytes, dgm::PlanarArgs& a) {
   char msg[128];
-  if (F < 1 || F > PB_MAX_FRAMES || P < 0 || W <= 0 || H <= 0 || R_cap < 0)
-    return snprintf(msg, sizeof(msg), "%s: bad size", who), bad(msg);
-  if (!planes || !geom_ws || !binning_ws || !img_ws || !planar_ws)
-    return snprintf(msg, sizeof(msg), "%s: null pointer", who), bad(msg);
-  if (F > 1) {
-    size_t gb, bb, ib;
-    dgr_workspace_sizes(P, W, H, R_cap, &gb, &bb, &ib);
-    if (geom_stride < gb || binning_stride < bb || img_stride < ib || geom_stride % 128 || binning_stride % 128 ||
-        img_stride % 128)
-      return snprintf(msg, sizeof(msg), "%s: workspace stride too small or not a multiple of 128", who), bad(msg);
-  }
+  a = {};
+  const int rc = forward_ws_args(who, PB_MAX_FRAMES, true, F, P, W, H, geom_ws, geom_stride, binning_ws,
+                                 binning_stride, R_cap, img_ws, img_stride, planes && planar_ws, a);
+  if (rc != DGM_OK) return rc;
   if (reinterpret_cast<uintptr_t>(planar_ws) % 16)
     return snprintf(msg, sizeof(msg), "%s: misaligned workspace", who), bad(msg);
   size_t need;
@@ -1044,12 +1043,7 @@ int planar_args(const char* who, int F, int P, int W, int H, const float* planes
     snprintf(g_last_error, sizeof(g_last_error), "%s: planar workspace too small", who);
     return DGM_E_WORKSPACE;
   }
-  a = {};
-  a.F = F, a.P = P, a.W = W, a.H = H, a.planes = planes;
-  a.geom_ws = geom_ws, a.binning_ws = binning_ws, a.img_ws = img_ws;
-  a.geom_stride = F > 1 ? geom_stride : 0, a.binning_stride = F > 1 ? binning_stride : 0;
-  a.img_stride = F > 1 ? img_stride : 0;
-  a.R_cap = R_cap, a.planar_ws = planar_ws;
+  a.planes = planes, a.planar_ws = planar_ws;
   return DGM_OK;
 }
 }  // namespace
@@ -1118,20 +1112,11 @@ int dgr_planar_bwd(int F, int P, int W, int H, const float* planes, void* geom_w
 int dgr_blend_stats(int F, int P, int W, int H, void* binning_ws, size_t binning_stride, int64_t R_cap,
                     void* img_ws, size_t img_stride, const float* pixel_weights, int weights_per_frame,
                     float* out_sum, float* out_max, void* stream) {
-  // grid.y counts the frames and is limited to 65535
-  if (F < 1 || F > 65535 || P < 0 || W < 1 || H < 1 || R_cap < 0) return bad("dgr_blend_stats: bad size");
-  if (!binning_ws || !img_ws || !out_sum || !out_max) return bad("dgr_blend_stats: null pointer");
-  if (F > 1) {
-    size_t gb, bb, ib;
-    dgr_workspace_sizes(P, W, H, R_cap, &gb, &bb, &ib);
-    if (binning_stride < bb || img_stride < ib || binning_stride % 128 || img_stride % 128)
-      return bad("dgr_blend_stats: workspace stride too small or not a multiple of 128");
-  }
   dgm::StatsArgs a = {};
-  a.F = F, a.P = P, a.W = W, a.H = H;
-  a.binning_ws = binning_ws, a.img_ws = img_ws;
-  a.binning_stride = F > 1 ? binning_stride : 0, a.img_stride = F > 1 ? img_stride : 0;
-  a.R_cap = R_cap;
+  // grid.y counts the frames and is limited to 65535
+  const int rc = forward_ws_args("dgr_blend_stats", 65535, false, F, P, W, H, nullptr, 0, binning_ws, binning_stride,
+                                 R_cap, img_ws, img_stride, out_sum && out_max, a);
+  if (rc != DGM_OK) return rc;
   a.pixel_weights = pixel_weights, a.weights_per_frame = (pixel_weights && weights_per_frame) ? 1 : 0;
   a.out_sum = out_sum, a.out_max = out_max;
   return check(dgm::launch_blend_stats(a, (cudaStream_t)stream));

@@ -91,9 +91,9 @@ __global__ void __launch_bounds__(256, 4) feature_fwd_kernel(int W, int H, int P
 // dL/dalpha_i += T_i sum_c (f_{i,c} - F_behind,c) dL/dF_c, walked front to back with the forward's T: the part of
 // the map behind record i is T_i F_behind = F - Pref_i, Pref_i the map's prefix through record i, accumulated
 // exactly as the forward accumulates the map, so dL/dalpha_i = sum_c dL/dF_c (T_i f_c - (F_c - Pref_i,c) / (1 - a)).
-// w = G dL/dG is staged with alpha T and contracted by contract_chunk<true> (dL/dF of the group's four channels
-// in its four rows): the six moments go to floats 0-5 of grad_acc (dL/dmean2D, dL/dconic, dL/dopacity, as the
-// blend backward forms them), the four weight sums to the feature accumulator of the frame (feat_ws + f ws_stride,
+// side_bwd_walk (raster_walk.cuh) contracts w = G dL/dG and alpha T with dL/dF of the group's four channels in its
+// four rows: the six moments go to floats 0-5 of grad_acc (dL/dmean2D, dL/dconic, dL/dopacity, as the blend
+// backward forms them), the four weight sums to the feature accumulator of the frame (feat_ws + f ws_stride,
 // [P, Cp] floats, Cp = C rounded up to 4).  Dynamic shared memory: STAGE_BYTES.
 __global__ void __launch_bounds__(256, 2) feature_bwd_kernel(int W, int H, int P, int C, char* geom_ws,
                                                              size_t geom_stride, const char* img_ws, size_t img_stride,
@@ -119,38 +119,27 @@ __global__ void __launch_bounds__(256, 2) feature_bwd_kernel(int W, int H, int P
   float4* const grad_acc = GeomWS::from(geom_ws + f * geom_stride, P).grad_acc;
   float* const facc = reinterpret_cast<float*>(feat_ws + f * ws_stride);
   const float* feats = features + (per_frame ? (size_t)f * P * C : 0);
-  const float cx = t.wx0 + 3.5f, cy = t.wy0 + 1.5f;  // centre of the warp's block
-  t.find_stops(&s_maxc, [&] {
-    for (int i = t.tid; i < RB * ACC_STRIDE; i += 256) s_acc[i] = 0.f;
-  });
-  if (t.maxc == 0) return;  // uniform per CTA
 
-  // the group's upstream gradient (the dL/dpixel rows of the contraction) and map values of this pixel
   float g[FG], Fm[FG], Pf[FG];
+  side_bwd_walk(
+      t, W, H, &s_maxc, s_geo, s_con, s_id, s_acc, s_dlp, s_stage, grad_acc,
+      [&] {  // the group's upstream gradient (the dL/dpixel rows of the contraction) and map values of this pixel
 #pragma unroll
-  for (int k = 0; k < FG; ++k) {
-    const bool ok = t.inside && c0 + k < C;
-    const size_t o = ((size_t)f * C + c0 + k) * npix + t.pix_id;
-    g[k] = ok ? dL_dfmap[o] : 0.0f;
-    Fm[k] = ok ? fmap[o] : 0.0f;
-    Pf[k] = 0.0f;
-    s_dlp[t.wid][k][t.lane] = g[k];
-  }
-  float* const stage = s_stage + t.wid * (CHUNK * SLOT_F);
-  int nslot = 0, rec = 0;  // staged records; the record of slot lane & 15
-  float T = 1.0f;
-
-  side_walk(
-      t, s_geo, s_con,
+        for (int k = 0; k < FG; ++k) {
+          const bool ok = t.inside && c0 + k < C;
+          const size_t o = ((size_t)f * C + c0 + k) * npix + t.pix_id;
+          g[k] = ok ? dL_dfmap[o] : 0.0f;
+          Fm[k] = ok ? fmap[o] : 0.0f;
+          Pf[k] = 0.0f;
+          s_dlp[t.wid][k][t.lane] = g[k];
+        }
+      },
       [&](int base, int cnt) {
         load_feature_batch(t.b, t.range.x + base, cnt, feats, C, c0, s_geo, s_con, s_f, t.tid);
         if ((int)t.tid < cnt)
           s_id[t.tid] = __float_as_uint(t.b.inst_attr[2 * ((size_t)t.range.x + base + t.tid) + 1].w);
       },
-      [&](int q, int j, float opac, float np, bool pre) {
-        const float G = expf(-np);
-        const float alpha = fminf(0.99f, __fmul_rn(opac, G));
-        const bool act = pre && !(alpha < 1.0f / 255.0f);
+      [&](int j, float alpha, float T, bool act) {
         const float4 fv = s_f[j];
         const float fa[FG] = {fv.x, fv.y, fv.z, fv.w};
         const float r1 = __fdividef(1.0f, 1.0f - alpha);
@@ -161,56 +150,9 @@ __global__ void __launch_bounds__(256, 2) feature_bwd_kernel(int W, int H, int P
           Pf[c] = act ? pn : Pf[c];
           dLa = fmaf(g[c], fmaf(T, fa[c], -(Fm[c] - Pf[c]) * r1), dLa);
         }
-        const float w = act ? (G * opac) * dLa : 0.0f;
-        const float aT = act ? alpha * T : 0.0f;
-        T = act ? __fmul_rn(T, __fadd_rn(1.0f, -alpha)) : T;
-        if (__any_sync(0xffffffffu, act)) {
-          stage[nslot * SLOT_F + t.lane] = w;
-          stage[nslot * SLOT_F + 32 + t.lane] = aT;
-          if ((int)(t.lane & 15) == nslot) rec = j;
-          ++nslot;
-        }
-        if (q == 1 && nslot > CHUNK - 2) {  // the pair is staged and there is no room for another
-          __syncwarp();
-          contract_chunk<true>(stage, &s_dlp[t.wid][0][0], nslot, rec, t.lane, s_geo, cx, cy, s_acc);
-          __syncwarp();
-          nslot = 0;
-        }
+        return dLa;
       },
-      [&](int cnt) {
-        if (nslot > 0) {  // the batch's records must be in s_acc before the flush
-          __syncwarp();
-          contract_chunk<true>(stage, &s_dlp[t.wid][0][0], nslot, rec, t.lane, s_geo, cx, cy, s_acc);
-          __syncwarp();
-          nslot = 0;
-        }
-        __syncthreads();
-        // ---- flush this batch: the moments as the blend backward turns them into gradients, and the feature sums
-        if ((int)t.tid < cnt) {
-          float* acc = &s_acc[t.tid * ACC_STRIDE];
-          float a[ACC_STRIDE];
-          bool nz = false;
-#pragma unroll
-          for (int q = 0; q < ACC_STRIDE; ++q) {
-            a[q] = acc[q];
-            nz |= (a[q] != 0.f);
-            acc[q] = 0.f;
-          }
-          if (nz) {
-            const float ddelx_dx = 0.5 * W;
-            const float ddely_dy = 0.5 * H;
-            const float4 con_o = s_con[t.tid];
-            const uint32_t id = s_id[t.tid];
-            const float g_mx = -ddelx_dx * (con_o.x * a[1] + con_o.y * a[2]);
-            const float g_my = -ddely_dy * (con_o.z * a[2] + con_o.y * a[1]);
-            const float g_op = (con_o.w != 0.0f) ? a[0] / con_o.w : 0.0f;
-            float* dst = reinterpret_cast<float*>(grad_acc + 3 * (size_t)id);
-            red_add_v4(dst, g_mx, g_my, -0.5f * a[3], -0.5f * a[4]);
-            red_add_v2(dst + 4, -0.5f * a[5], g_op);
-            red_add_v4(facc + (size_t)id * Cp + c0, a[6], a[7], a[8], a[9]);
-          }
-        }
-      });
+      [&](int, uint32_t id, const float* a) { red_add_v4(facc + (size_t)id * Cp + c0, a[6], a[7], a[8], a[9]); });
 }
 
 // dL/dfeatures from the feature accumulators of F frames, one thread per (Gaussian, padded channel): per_frame,
@@ -258,12 +200,7 @@ cudaError_t launch_features_fwd(const FeatArgs& a, cudaStream_t s) {
 }
 
 cudaError_t launch_features_bwd(const FeatArgs& a, cudaStream_t s) {
-  static unsigned long long attr = 0;  // per device
-  if (once_per_device(attr)) {
-    cudaFuncSetAttribute(feature_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, STAGE_BYTES);
-    cudaFuncSetAttribute(feature_bwd_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                         cudaSharedmemCarveoutMaxShared);
-  }
+  side_bwd_attributes<feature_bwd_kernel>();
   if (a.P == 0) return cudaSuccess;
   const unsigned gx = (a.W + TILE_X - 1) / TILE_X, gy = (a.H + TILE_Y - 1) / TILE_Y;
   const size_t stride = feature_ws_stride(a.P, a.C);

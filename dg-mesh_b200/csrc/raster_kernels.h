@@ -92,18 +92,22 @@ struct BwdArgs {
 };
 #define PB_MAX_FRAMES 64
 
-// feature maps (raster_feat.cu): a pass over the workspaces of F frames an earlier forward wrote (frame f's at
-// geom_ws + f * geom_stride, ...).  features [P,C], or [F,P,C] with per_frame; out_map / map / dL_dmap [F,C,H,W].
-// feat_ws holds F per-Gaussian accumulators of dL/dfeatures, feature_ws_stride(P, C) bytes apart: the forward
-// clears them, the backward adds into them and launch_features_bwd's finish re-zeroes them while it writes
-// dL_dfeatures ([F,P,C] with per_frame, else the [P,C] sum over the frames; NULL: only re-zeroes)
-struct FeatArgs {
-  int F, P, C, W, H;
-  const float* features;
-  int per_frame;
+// The workspaces of F frames an earlier forward wrote, which a side pass (features, planar depth, blend statistics)
+// reads: frame f's at geom_ws + f * geom_stride, ... (strides 0 for one frame; blend statistics reads no geom_ws)
+struct ForwardWS {
+  int F, P, W, H;
   void *geom_ws, *binning_ws, *img_ws;
   size_t geom_stride, binning_stride, img_stride;
   int64_t R_cap;
+};
+// feature maps (raster_feat.cu): features [P,C], or [F,P,C] with per_frame; out_map / map / dL_dmap [F,C,H,W].
+// feat_ws holds F per-Gaussian accumulators of dL/dfeatures, feature_ws_stride(P, C) bytes apart: the forward
+// clears them, the backward adds into them and launch_features_bwd's finish re-zeroes them while it writes
+// dL_dfeatures ([F,P,C] with per_frame, else the [P,C] sum over the frames; NULL: only re-zeroes)
+struct FeatArgs : ForwardWS {
+  int C;
+  const float* features;
+  int per_frame;
   float* out_map;           // forward
   const float *map, *dL_dmap;  // backward
   float* dL_dfeatures;      // backward
@@ -112,14 +116,9 @@ struct FeatArgs {
 size_t feature_ws_stride(int P, int C);
 cudaError_t launch_features_fwd(const FeatArgs& a, cudaStream_t s);  // raster_feat.cu
 cudaError_t launch_features_bwd(const FeatArgs& a, cudaStream_t s);  // raster_feat.cu
-// blend-weight statistics (raster_stats.cu): a pass over the binning / img workspaces of F frames an earlier forward
-// wrote (frame f's at binning_ws + f * binning_stride, ...).  pixel_weights NULL, [H,W] or, with weights_per_frame,
-// [F,H,W]; out_sum / out_max [F,P], zeroed by the launch
-struct StatsArgs {
-  int F, P, W, H;
-  void *binning_ws, *img_ws;
-  size_t binning_stride, img_stride;
-  int64_t R_cap;
+// blend-weight statistics (raster_stats.cu): pixel_weights NULL, [H,W] or, with weights_per_frame, [F,H,W];
+// out_sum / out_max [F,P], zeroed by the launch
+struct StatsArgs : ForwardWS {
   const float* pixel_weights;
   int weights_per_frame;
   float *out_sum, *out_max;
@@ -143,15 +142,10 @@ struct PlaneArgs {
 };
 cudaError_t launch_gaussian_planes_fwd(const PlaneArgs& a, cudaStream_t s);  // gaussian_planes.cu
 cudaError_t launch_gaussian_planes_bwd(const PlaneArgs& a, cudaStream_t s);  // gaussian_planes.cu
-// planar-depth maps (raster_planar.cu): a pass over the workspaces of F frames an earlier forward wrote, like
-// FeatArgs.  planes [F,P,3]; maps [F,1,H,W]; planar_ws holds F per-frame workspaces planar_ws_stride(P, W, H) bytes
-// apart (a plane accumulator per Gaussian and the median record per pixel)
-struct PlanarArgs {
-  int F, P, W, H;
+// planar-depth maps (raster_planar.cu): planes [F,P,3]; maps [F,1,H,W]; planar_ws holds F per-frame workspaces
+// planar_ws_stride(P, W, H) bytes apart (a plane accumulator per Gaussian and the median record per pixel)
+struct PlanarArgs : ForwardWS {
   const float* planes;
-  void *geom_ws, *binning_ws, *img_ws;
-  size_t geom_stride, binning_stride, img_stride;
-  int64_t R_cap;
   float *out_depth, *out_median;                     // forward
   const float *depth, *dL_ddepth, *dL_dmedian;       // backward (each gradient may be NULL)
   float* dL_dplanes;                                 // backward

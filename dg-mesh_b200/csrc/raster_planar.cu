@@ -106,10 +106,11 @@ __global__ void __launch_bounds__(256, 4) planar_fwd_kernel(int W, int H, int P,
   }
 }
 
-// dL/dalpha_i += dL/dD (T_i d_i(p) - (D - Pref_i) / (1 - alpha_i)), walked front to back with the forward's T as
-// feature_bwd_kernel walks it.  The four dL/dpixel rows of contract_chunk<true> are dL/dD, dL/dD u', dL/dD v', 0 with
-// (u', v') = p minus the TILE's centre (the warps' sums meet in one per-tile accumulator, so their offsets must share
-// an origin); at the flush sum e (p - mu) = (S_u' - Gx' S, S_v' - Gy' S), (Gx', Gy') = mu minus the tile's centre.
+// dL/dalpha_i += dL/dD (T_i d_i(p) - (D - Pref_i) / (1 - alpha_i)), walked front to back with the forward's T by
+// side_bwd_walk (raster_walk.cuh), as feature_bwd_kernel is.  The four dL/dpixel rows of contract_chunk<true> are
+// dL/dD, dL/dD u', dL/dD v', 0 with (u', v') = p minus the TILE's centre (the warps' sums meet in one per-tile
+// accumulator, so their offsets must share an origin); at the flush sum e (p - mu) = (S_u' - Gx' S, S_v' - Gy' S),
+// (Gx', Gy') = mu minus the tile's centre.
 __global__ void __launch_bounds__(256, 2) planar_bwd_kernel(int W, int H, int P, char* geom_ws, size_t geom_stride,
                                                             const char* img_ws, size_t img_stride, const char* bin_ws,
                                                             size_t bin_stride, int64_t R_cap,
@@ -133,87 +134,34 @@ __global__ void __launch_bounds__(256, 2) planar_bwd_kernel(int W, int H, int P,
   float4* const grad_acc = GeomWS::from(geom_ws + f * geom_stride, P).grad_acc;
   float4* const pacc = PlanarWS::from(pl_ws + f * ws_stride, P).acc;
   const float* pl = planes + (size_t)f * P * 3;
-  const float cx = t.wx0 + 3.5f, cy = t.wy0 + 1.5f;  // centre of the warp's block
   const unsigned gx = (W + TILE_X - 1) / TILE_X;
   const float tcx = (t.tile % gx) * TILE_X + 0.5f * (TILE_X - 1), tcy = (t.tile / gx) * TILE_Y + 0.5f * (TILE_Y - 1);
   const float px = -t.npx2.x, py = -t.npy2.x;
-  t.find_stops(&s_maxc, [&] {
-    for (int i = t.tid; i < RB * ACC_STRIDE; i += 256) s_acc[i] = 0.f;
-  });
-  if (t.maxc == 0) return;  // uniform per CTA
 
-  const size_t o = (size_t)f * npix + t.pix_id;
-  const float g = t.inside ? dL_ddmap[o] : 0.0f, Dm = t.inside ? dmap[o] : 0.0f;
-  s_dlp[t.wid][0][t.lane] = g;
-  s_dlp[t.wid][1][t.lane] = g * (px - tcx);
-  s_dlp[t.wid][2][t.lane] = g * (py - tcy);
-  s_dlp[t.wid][3][t.lane] = 0.0f;
-  float* const stage = s_stage + t.wid * (CHUNK * SLOT_F);
-  int nslot = 0, rec = 0;
-  float T = 1.0f, Pf = 0.0f;
-
-  side_walk(
-      t, s_geo, s_con,
+  float g, Dm, Pf = 0.0f;
+  side_bwd_walk(
+      t, W, H, &s_maxc, s_geo, s_con, s_id, s_acc, s_dlp, s_stage, grad_acc,
+      [&] {
+        const size_t o = (size_t)f * npix + t.pix_id;
+        g = t.inside ? dL_ddmap[o] : 0.0f, Dm = t.inside ? dmap[o] : 0.0f;
+        s_dlp[t.wid][0][t.lane] = g;
+        s_dlp[t.wid][1][t.lane] = g * (px - tcx);
+        s_dlp[t.wid][2][t.lane] = g * (py - tcy);
+        s_dlp[t.wid][3][t.lane] = 0.0f;
+      },
       [&](int base, int cnt) { load_planar_batch(t.b, t.range.x + base, cnt, pl, s_geo, s_con, s_pl, s_id, t.tid); },
-      [&](int q, int j, float opac, float np, bool pre) {
-        const float G = expf(-np);
-        const float alpha = fminf(0.99f, __fmul_rn(opac, G));
-        const bool act = pre && !(alpha < 1.0f / 255.0f);
+      [&](int j, float alpha, float T, bool act) {
         const float d = plane_depth(s_pl[j], s_geo[j], px, py);
         const float r1 = __fdividef(1.0f, 1.0f - alpha);
         const float pn = __fmaf_rn(T, __fmul_rn(alpha, d), Pf);
         Pf = act ? pn : Pf;
-        const float dLa = g * fmaf(T, d, -(Dm - Pf) * r1);
-        const float w = act ? (G * opac) * dLa : 0.0f;
-        const float aT = act ? alpha * T : 0.0f;
-        T = act ? __fmul_rn(T, __fadd_rn(1.0f, -alpha)) : T;
-        if (__any_sync(0xffffffffu, act)) {
-          stage[nslot * SLOT_F + t.lane] = w;
-          stage[nslot * SLOT_F + 32 + t.lane] = aT;
-          if ((int)(t.lane & 15) == nslot) rec = j;
-          ++nslot;
-        }
-        if (q == 1 && nslot > CHUNK - 2) {
-          __syncwarp();
-          contract_chunk<true>(stage, &s_dlp[t.wid][0][0], nslot, rec, t.lane, s_geo, cx, cy, s_acc);
-          __syncwarp();
-          nslot = 0;
-        }
+        return g * fmaf(T, d, -(Dm - Pf) * r1);
       },
-      [&](int cnt) {
-        if (nslot > 0) {
-          __syncwarp();
-          contract_chunk<true>(stage, &s_dlp[t.wid][0][0], nslot, rec, t.lane, s_geo, cx, cy, s_acc);
-          __syncwarp();
-          nslot = 0;
-        }
-        __syncthreads();
-        if ((int)t.tid < cnt) {
-          float* acc = &s_acc[t.tid * ACC_STRIDE];
-          float a[ACC_STRIDE];
-          bool nz = false;
-#pragma unroll
-          for (int k = 0; k < ACC_STRIDE; ++k) {
-            a[k] = acc[k];
-            nz |= (a[k] != 0.f);
-            acc[k] = 0.f;
-          }
-          if (nz) {
-            const float ddelx_dx = 0.5 * W;
-            const float ddely_dy = 0.5 * H;
-            const float4 con_o = s_con[t.tid];
-            const float4 ge = s_geo[t.tid], p4 = s_pl[t.tid];
-            const uint32_t id = s_id[t.tid];
-            const float g_mx = -ddelx_dx * (con_o.x * a[1] + con_o.y * a[2] + p4.y * a[6]);
-            const float g_my = -ddely_dy * (con_o.z * a[2] + con_o.y * a[1] + p4.z * a[6]);
-            const float g_op = (con_o.w != 0.0f) ? a[0] / con_o.w : 0.0f;
-            float* dst = reinterpret_cast<float*>(grad_acc + 3 * (size_t)id);
-            red_add_v4(dst, g_mx, g_my, -0.5f * a[3], -0.5f * a[4]);
-            red_add_v2(dst + 4, -0.5f * a[5], g_op);
-            red_add_v4(reinterpret_cast<float*>(pacc + id), a[6], fmaf(-(ge.x - tcx), a[6], a[7]),
-                       fmaf(-(ge.y - tcy), a[6], a[8]), 0.0f);
-          }
-        }
+      [&](int r, uint32_t id, const float* a) {  // the plane sums, and -g sum e for dL/dmean2D
+        const float4 ge = s_geo[r], p4 = s_pl[r];
+        red_add_v4(reinterpret_cast<float*>(pacc + id), a[6], fmaf(-(ge.x - tcx), a[6], a[7]),
+                   fmaf(-(ge.y - tcy), a[6], a[8]), 0.0f);
+        return make_float2(p4.y * a[6], p4.z * a[6]);
       });
 }
 
@@ -273,12 +221,7 @@ cudaError_t launch_planar_fwd(const PlanarArgs& a, cudaStream_t s) {
 }
 
 cudaError_t launch_planar_bwd(const PlanarArgs& a, cudaStream_t s) {
-  static unsigned long long attr = 0;  // per device
-  if (once_per_device(attr)) {
-    cudaFuncSetAttribute(planar_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, STAGE_BYTES);
-    cudaFuncSetAttribute(planar_bwd_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                         cudaSharedmemCarveoutMaxShared);
-  }
+  side_bwd_attributes<planar_bwd_kernel>();
   if (a.P == 0) return cudaSuccess;
   const unsigned gx = (a.W + TILE_X - 1) / TILE_X, gy = (a.H + TILE_Y - 1) / TILE_Y;
   const size_t stride = planar_ws_stride(a.P, a.W, a.H);

@@ -1,9 +1,10 @@
-// raster_walk.cuh -- the walk of the side passes (feature_fwd_kernel, feature_bwd_kernel in raster_feat.cu,
-// blend_stats_kernel in raster_stats.cu): passes over the workspaces an existing forward left behind (sorted blend
-// records, tile ranges, tile order, n_contrib).  The walk repeats the forward's blend operation for operation (same
-// quadratic form, alpha, 1/255 skip and stop at n_contrib), so the transmittance a side pass sees is the forward's
-// bit for bit.
+// raster_walk.cuh -- the walk of the side passes (the feature kernels in raster_feat.cu, the planar kernels in
+// raster_planar.cu, blend_stats_kernel in raster_stats.cu): passes over the workspaces an existing forward left
+// behind (sorted blend records, tile ranges, tile order, n_contrib).  The walk repeats the forward's blend operation
+// for operation (same quadratic form, alpha, 1/255 skip and stop at n_contrib), so the transmittance a side pass sees
+// is the forward's bit for bit.  The side passes' backward kernels share side_bwd_walk on top of it.
 #pragma once
+#include <type_traits>
 #include "raster_bwd_blend.cuh"
 
 namespace dgm {
@@ -102,6 +103,109 @@ __device__ __forceinline__ void side_walk(const SideTile& t, const float4* s_geo
       }
     }
     end(cnt);
+  }
+}
+
+// The backward walk of a side pass (feature_bwd_kernel, planar_bwd_kernel), called by the whole CTA: side_walk with
+// the forward's T and its branch-free alpha / 1/255 gate.  Each warp stages w = G dL/dG and alpha T of the records
+// it blends in its CHUNK slots of s_stage (STAGE_BYTES of dynamic shared memory) and contracts them with its four
+// dL/dpixel rows s_dlp[wid] (contract_chunk<true>) when a pair leaves no room for another and at the batch's end.
+// After the batch's barrier each record's six moments go to floats 0-5 of grad_acc, as the blend backward turns them
+// into dL/dmean2D, dL/dconic and dL/dopacity.  A CTA whose pixels blend nothing returns before rows().
+//   rows()                     the warp's dL/dpixel rows into s_dlp[wid], and the per-pixel values dla reads
+//   stage(base, cnt)           as side_walk's, and each record's Gaussian id into s_id
+//   dla(j, alpha, T, act)      dL/dalpha of record j at the pixel; advances the kernel's prefix of its map when act
+//                              (the pixel blends the record)
+//   flush(r, id, a)            adds record r's own totals a[6..9] into the kernel's accumulator; returns void, or a
+//                              float2 that the flush adds to dL/dmean2D's two sums before their W/2, H/2 scale
+template <class Rows, class Stage, class DLa, class Flush>
+__device__ __forceinline__ void side_bwd_walk(SideTile& t, int W, int H, int* s_maxc, const float4* s_geo,
+                                              const float4* s_con, const uint32_t* s_id, float* s_acc,
+                                              float (*s_dlp)[4][32], float* s_stage, float4* grad_acc, Rows rows,
+                                              Stage stage, DLa dla, Flush flush) {
+  constexpr int ACC_STRIDE = acc_stride<true>();
+  const float cx = t.wx0 + 3.5f, cy = t.wy0 + 1.5f;  // centre of the warp's block
+  t.find_stops(s_maxc, [&] {
+    for (int i = t.tid; i < RB * ACC_STRIDE; i += 256) s_acc[i] = 0.f;
+  });
+  if (t.maxc == 0) return;  // uniform per CTA
+  rows();
+  float* const stg = s_stage + t.wid * (CHUNK * SLOT_F);
+  int nslot = 0, rec = 0;  // staged records; the record of slot lane & 15
+  float T = 1.0f;
+
+  side_walk(
+      t, s_geo, s_con, stage,
+      [&](int q, int j, float opac, float np, bool pre) {
+        const float G = expf(-np);
+        const float alpha = fminf(0.99f, __fmul_rn(opac, G));
+        const bool act = pre && !(alpha < 1.0f / 255.0f);
+        const float dLa = dla(j, alpha, T, act);
+        const float w = act ? (G * opac) * dLa : 0.0f;
+        const float aT = act ? alpha * T : 0.0f;
+        T = act ? __fmul_rn(T, __fadd_rn(1.0f, -alpha)) : T;
+        if (__any_sync(0xffffffffu, act)) {
+          stg[nslot * SLOT_F + t.lane] = w;
+          stg[nslot * SLOT_F + 32 + t.lane] = aT;
+          if ((int)(t.lane & 15) == nslot) rec = j;
+          ++nslot;
+        }
+        if (q == 1 && nslot > CHUNK - 2) {  // the pair is staged and there is no room for another
+          __syncwarp();
+          contract_chunk<true>(stg, &s_dlp[t.wid][0][0], nslot, rec, t.lane, s_geo, cx, cy, s_acc);
+          __syncwarp();
+          nslot = 0;
+        }
+      },
+      [&](int cnt) {
+        if (nslot > 0) {  // the batch's records must be in s_acc before the flush
+          __syncwarp();
+          contract_chunk<true>(stg, &s_dlp[t.wid][0][0], nslot, rec, t.lane, s_geo, cx, cy, s_acc);
+          __syncwarp();
+          nslot = 0;
+        }
+        __syncthreads();
+        // ---- flush this batch: the moments as the blend backward turns them into gradients, and the kernel's sums
+        if ((int)t.tid < cnt) {
+          float* acc = &s_acc[t.tid * ACC_STRIDE];
+          float a[ACC_STRIDE];
+          bool nz = false;
+#pragma unroll
+          for (int q = 0; q < ACC_STRIDE; ++q) {
+            a[q] = acc[q];
+            nz |= (a[q] != 0.f);
+            acc[q] = 0.f;
+          }
+          if (nz) {
+            const float ddelx_dx = 0.5 * W;
+            const float ddely_dy = 0.5 * H;
+            const float4 con_o = s_con[t.tid];
+            const uint32_t id = s_id[t.tid];
+            float sx = con_o.x * a[1] + con_o.y * a[2], sy = con_o.z * a[2] + con_o.y * a[1];
+            if constexpr (std::is_void_v<decltype(flush(t.tid, id, a))>) {
+              flush(t.tid, id, a);
+            } else {
+              const float2 m = flush(t.tid, id, a);
+              sx += m.x, sy += m.y;
+            }
+            const float g_mx = -ddelx_dx * sx;
+            const float g_my = -ddely_dy * sy;
+            const float g_op = (con_o.w != 0.0f) ? a[0] / con_o.w : 0.0f;
+            float* dst = reinterpret_cast<float*>(grad_acc + 3 * (size_t)id);
+            red_add_v4(dst, g_mx, g_my, -0.5f * a[3], -0.5f * a[4]);
+            red_add_v2(dst + 4, -0.5f * a[5], g_op);
+          }
+        }
+      });
+}
+
+// a side-pass backward kernel's launch attributes, once per device: the staging areas' STAGE_BYTES of dynamic
+// shared memory and the largest shared-memory carveout
+template <auto Kernel> void side_bwd_attributes() {
+  static unsigned long long attr = 0;  // per device
+  if (once_per_device(attr)) {
+    cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, STAGE_BYTES);
+    cudaFuncSetAttribute(Kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   }
 }
 
