@@ -25,6 +25,7 @@ Differences that are deliberate (DESIGN.md):
   * work is enqueued on the CURRENT torch stream (the reference uses the legacy
     default stream).
 """
+import copy
 import os
 import struct
 import sys
@@ -172,27 +173,57 @@ def _sizes(P, W, H, R_cap):
 
 
 class _Workspace:
-    """geom | binning | img | status carved from ONE device allocation (the three opaque buffers
-    of the reference, dgr/rasterize_points.cu:68-78, kept together for the backward pass)."""
-    __slots__ = ("buf", "geom", "binning", "img", "status", "gb", "bb", "ib", "R_cap", "nrm", "surf")
+    """The workspaces of F frames: geom | binning | img of every frame, then the F status blocks, carved from ONE
+    device allocation (the three opaque buffers of the reference, dgr/rasterize_points.cu:68-78, kept together for
+    the backward pass), and the normal and surface workspaces of a forward that writes those maps.  Frame f's buffers
+    start f strides in (gs, bs, is_, nrm_stride, surf_stride: the sizes rounded up to 512 bytes).  The single-frame
+    entry points take the exact sizes gb, bb, ib, nrm_bytes and surf_bytes; the batch ones take the strides.
+    `batch`: the workspace of a batch call, whose status words have a leading frame dimension even for F = 1."""
+    __slots__ = ("buf", "geom", "binning", "img", "status", "gb", "bb", "ib", "gs", "bs", "is_", "R_cap", "F", "lead",
+                 "nrm", "nrm_bytes", "nrm_stride", "surf", "surf_bytes", "surf_stride")
 
-    def __init__(self, P, W, H, R_cap, dev):
-        gb, bb, ib, ga, ba, ia = _sizes(P, W, H, R_cap)
-        self.buf = torch.empty((ga + ba + ia + 64,), dtype=torch.uint8, device=dev)
+    def __init__(self, F, P, W, H, R_cap, dev, batch=False, normal=False, surface=False):
+        self.gb, self.bb, self.ib, self.gs, self.bs, self.is_ = _sizes(P, W, H, R_cap)
+        self.buf = torch.empty((F * (self.gs + self.bs + self.is_ + 32),), dtype=torch.uint8, device=dev)
         base = self.buf.data_ptr()
-        self.geom, self.binning, self.img, self.status = base, base + ga, base + ga + ba, base + ga + ba + ia
-        self.gb, self.bb, self.ib, self.R_cap = gb, bb, ib, R_cap
-        self.nrm = None     # the normal workspace of a normal forward (_normal_ws)
-        self.surf = None    # the surface workspace of a surface forward
+        self.geom, self.binning, self.img = base, base + F * self.gs, base + F * (self.gs + self.bs)
+        self.status = self.img + F * self.is_
+        self.R_cap, self.F, self.lead = R_cap, F, ((F,) if batch else ())
+        self.nrm, self.nrm_bytes, self.nrm_stride = _side_ws(F, _normal_ws_bytes(P, R_cap), dev) if normal else \
+            (None, 0, 0)
+        self.surf, self.surf_bytes, self.surf_stride = _side_ws(F, _surface_ws_bytes(W, H), dev) if surface else \
+            (None, 0, 0)
 
     def status_tensor(self):
-        return self.buf[-64:-32].view(torch.int32)
+        """The status words: [8] for a single-frame call, [F,8] for a batch."""
+        o = self.status - self.buf.data_ptr()
+        return self.buf[o:o + 32 * self.F].view(torch.int32).view(self.lead + (8,))
 
-    # the reference-style separate byte tensors (views, no copies)
+    def side_args(self):
+        """(geom, stride, binning, stride, R_cap, img, stride) of the passes over this forward's blend (features,
+        planar depth, blend statistics); the strides are 0 for a single-frame call."""
+        if self.lead:
+            return self.geom, self.gs, self.binning, self.bs, self.R_cap, self.img, self.is_
+        return self.geom, 0, self.binning, 0, self.R_cap, self.img, 0
+
+    def frame(self, f):
+        """Frame f of a batch as a single-frame workspace over the same allocation (for export_state)."""
+        w = copy.copy(self)
+        w.geom, w.binning, w.img = self.geom + f * self.gs, self.binning + f * self.bs, self.img + f * self.is_
+        w.status, w.F, w.lead = self.status + 32 * f, 1, ()
+        return w
+
+    # the reference-style separate byte tensors of a single frame (views, no copies)
     def split(self):
         o1 = self.binning - self.geom
         o2 = self.img - self.geom
         return self.buf[:self.gb], self.buf[o1:o1 + self.bb], self.buf[o2:o2 + self.ib]
+
+
+def _side_ws(F, nbytes, dev):
+    """(buffer, nbytes, stride) of F side workspaces of nbytes each."""
+    stride = (nbytes + 511) // 512 * 512
+    return torch.empty((F * stride,), dtype=torch.uint8, device=dev), nbytes, stride
 
 
 def _normal_ws_bytes(P, R_cap):
@@ -243,41 +274,113 @@ def _null_segment(name, narrower, at):
     return v
 
 
-def _raw_forward(bg, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
-                 projmatrix, tan_fovx, tan_fovy, H, W, sh, degree, campos, prefiltered, R_cap, notify=None,
-                 lo=0.0, hi=0.0, out=None, max_tile=0, maps=None, nrm=None, surf=None):
-    """One enqueue of the dgr_forward entry point (see `_enqueue`) that also writes `maps` = (depth, alpha) [1,H,W]
-    and, with the maps, `nrm` = (normals [P,3], normal map [3,H,W]) and `surf` = (near, far, median [1,H,W],
-    distortion [1,H,W]).  Returns (color, radii, workspace)."""
-    if means3D.ndim != 2 or means3D.shape[1] != 3:
+def _forward(batch, settings, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, maps=None,
+             nrm=None, surf=None, cams=None, attempt=None):
+    """Enqueue the forward of the frames of `settings` (a tuple of them with `batch`, else one) through the narrowest
+    dgr_forward or dgr_forward_batch variant (see `_enqueue`) that also writes
+      maps: None, or the (depth, alpha) maps [1,H,W] ([F,1,H,W] with `batch`);
+      nrm: None, or (normals [P,3] (with `batch` also [F,P,3] per frame), normal maps [3,H,W] / [F,3,H,W]);
+      surf: None, or (near, far, median-depth maps, distortion maps), each map as the depth map.
+    The Gaussian inputs are [P,.], or with `batch` [F,P,.] per frame where their rank says so.  cams: None (the
+    settings' cameras), or the (viewmatrix, projmatrix, campos) tensors to use instead, stacked with `batch`.  A frame
+    that did not fit the instance workspace is re-run into the outputs of the first attempt (`_run_sized`); with
+    `attempt` = (R_cap, notify, depth hint lo, hi) the forward is enqueued once, as given, and R is None.
+    Returns (color, radii, workspace, R of the largest frame (None under stream capture), (means3D, the other inputs
+    as the library reads them (bg, sh, colors, opacities, scales, rotations, cov3D, view, proj, campos), their
+    (tanfovx, tanfovy), the per-frame mask))."""
+    rs0 = settings[0] if batch else settings
+    F = len(settings) if batch else 1
+    if batch:
+        if F > _MAX_FRAMES:
+            raise ValueError(f"at most {_MAX_FRAMES} frames per batch")
+        for s in settings:
+            if (s.image_height, s.image_width, s.sh_degree, s.scale_modifier) != \
+                    (rs0.image_height, rs0.image_width, rs0.sh_degree, rs0.scale_modifier):
+                raise ValueError("all frames of a batch must share image size, SH degree and scale modifier")
+    means3D = _f32c(means3D, "means3D")
+    if means3D is None:
+        raise ValueError("means3D must have dimensions (num_points, 3)")
+    bg, sh, col, opac, sc, rot, cov = (
+        _f32c(rs0.bg, "bg"), _f32c(sh, "sh"), _f32c(colors_precomp, "colors_precomp"), _f32c(opacities, "opacities"),
+        _f32c(scales, "scales"), _f32c(rotations, "rotations"), _f32c(cov3Ds_precomp, "cov3D_precomp"))
+    pf = 0
+    if batch:
+        # per-frame mask from the ranks: means [F,P,3], scales [F,P,3], rotations [F,P,4], opacities [F,P,1],
+        # shs [F,P,M,3] / colors [F,P,3], cov3D [F,P,6]
+        for x, rank, bit in ((means3D, 3, _PF_MEANS), (sc, 3, _PF_SCALES), (rot, 3, _PF_ROTS), (opac, 3, _PF_OPAC),
+                             (sh, 4, _PF_COLOR), (col, 3, _PF_COLOR), (cov, 3, _PF_COV)):
+            if x is not None and x.ndim == rank:
+                if x.shape[0] != F:
+                    raise ValueError("per-frame inputs must have a leading dimension equal to the number of frames")
+                pf |= bit
+    if means3D.shape[-1] != 3 or not batch and means3D.ndim != 2:
         raise ValueError("means3D must have dimensions (num_points, 3)")  # rasterize_points.cu:57-59
     dev = means3D.device
-    P = means3D.shape[0]
-    M = int(sh.shape[1]) if (sh is not None and sh.numel() != 0) else 0
-    ws = _Workspace(P, W, H, R_cap, dev)
-    if out is None:
-        color = torch.empty((3, H, W), dtype=torch.float32, device=dev)
-        radii = torch.empty((P,), dtype=torch.int32, device=dev)
+    if cams is not None:
+        view, proj, campos = (_f32c(t.detach(), n) for t, n in zip(cams, ("viewmatrix", "projmatrix", "campos")))
+        tx, ty = _fovs(settings) if batch else (rs0.tanfovx, rs0.tanfovy)
+    elif batch:
+        view, proj, campos, tx, ty = _stack_settings(settings, dev)
     else:
-        color, radii = out      # a re-run after an overflow writes the tensors of the first attempt
+        view, proj, campos = (_f32c(rs0.viewmatrix, "viewmatrix"), _f32c(rs0.projmatrix, "projmatrix"),
+                              _f32c(rs0.campos, "campos"))
+        tx, ty = rs0.tanfovx, rs0.tanfovy
+    P = means3D.shape[-2]
+    H, W = int(rs0.image_height), int(rs0.image_width)
+    M = int(sh.shape[-2]) if sh is not None else 0
+    lead = (F,) if batch else ()
     p = _dgm_lib.ptr
-    head = (P, degree, M, p(bg), W, H, p(means3D), p(sh), p(colors), p(opacity), p(scales), float(scale_modifier),
-            p(rotations), p(cov3D_precomp), p(viewmatrix), p(projmatrix), p(campos), float(tan_fovx),
-            float(tan_fovy), int(bool(prefiltered)), p(color), p(radii))
-    tail = (ws.geom, ws.gb, ws.binning, ws.bb, R_cap, ws.img, ws.ib, ws.status,
-            notify.host_ptr if notify else None, notify.event if notify else None, lo, hi, int(max_tile),
-            _dgm_lib.stream_ptr())
-    nrm_args = surf_args = None
-    if nrm is not None:
-        nb = _normal_ws_bytes(P, R_cap)
-        ws.nrm = torch.empty((nb,), dtype=torch.uint8, device=dev)
-        nrm_args = (p(nrm[0]), p(nrm[1]), ws.nrm.data_ptr(), nb)
-    if surf is not None:
-        sb = _surface_ws_bytes(W, H)
-        ws.surf = torch.empty((sb,), dtype=torch.uint8, device=dev)
-        surf_args = (float(surf[0]), float(surf[1]), p(surf[2]), p(surf[3]), ws.surf.data_ptr(), sb)
-    _enqueue("dgr_forward", ((None, head), ("_aux", None if maps is None else (p(maps[0]), p(maps[1]))),
-                             ("_nrm", nrm_args), ("_surf", surf_args), (None, tail)))
+    npf = int(nrm is not None and nrm[0].ndim == 3)
+    first = []
+
+    def run(R_cap, notify, lo, hi, mt):
+        ws = _Workspace(F, P, W, H, R_cap, dev, batch, nrm is not None, surf is not None)
+        if not first:    # a re-run after an overflow writes the tensors of the first attempt
+            first.append((torch.empty(lead + (3, H, W), dtype=torch.float32, device=dev),
+                          torch.empty(lead + (P,), dtype=torch.int32, device=dev)))
+        color, radii = first[0]
+        note = (notify.host_ptr, notify.event) if notify else (None, None)
+        nrm_ws = None if nrm is None else ws.nrm.data_ptr()
+        surf_ws = None if surf is None else ws.surf.data_ptr()
+        if batch:
+            head = (F, P, rs0.sh_degree, M, p(bg), W, H, p(means3D), p(sh), p(col), p(opac), p(sc),
+                    float(rs0.scale_modifier), p(rot), p(cov), pf, p(view), p(proj), p(campos), tx, ty,
+                    int(bool(rs0.prefiltered)), p(color), p(radii))
+            tail = (ws.geom, ws.gs, ws.binning, ws.bs, R_cap, ws.img, ws.is_, ws.status, *note, lo, hi, int(mt),
+                    _N_STREAMS, _dgm_lib.stream_ptr())
+            nrm_args = None if nrm is None else (p(nrm[0]), npf, p(nrm[1]), nrm_ws, ws.nrm_stride)
+            surf_bytes = ws.surf_stride
+        else:
+            head = (P, rs0.sh_degree, M, p(bg), W, H, p(means3D), p(sh), p(col), p(opac), p(sc),
+                    float(rs0.scale_modifier), p(rot), p(cov), p(view), p(proj), p(campos), float(tx), float(ty),
+                    int(bool(rs0.prefiltered)), p(color), p(radii))
+            tail = (ws.geom, ws.gb, ws.binning, ws.bb, R_cap, ws.img, ws.ib, ws.status, *note, lo, hi, int(mt),
+                    _dgm_lib.stream_ptr())
+            nrm_args = None if nrm is None else (p(nrm[0]), p(nrm[1]), nrm_ws, ws.nrm_bytes)
+            surf_bytes = ws.surf_bytes
+        _enqueue("dgr_forward_batch" if batch else "dgr_forward", (
+            (None, head), ("_aux", None if maps is None else (p(maps[0]), p(maps[1]))), ("_nrm", nrm_args),
+            ("_surf", None if surf is None else (float(surf[0]), float(surf[1]), p(surf[2]), p(surf[3]), surf_ws,
+                                                 surf_bytes)),
+            (None, tail)))
+        return color, radii, ws
+
+    if attempt is not None:
+        (color, radii, ws), R = run(*attempt, 0), None
+    else:
+        (color, radii, ws), R = _run_sized(run, (dev.index, W, H), P, dev.index, F)
+    return color, radii, ws, R, (means3D, (bg, sh, col, opac, sc, rot, cov, view, proj, campos), (tx, ty), pf)
+
+
+def _raw_forward(bg, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
+                 projmatrix, tan_fovx, tan_fovy, H, W, sh, degree, campos, prefiltered, R_cap, notify=None, lo=0.0,
+                 hi=0.0):
+    """One enqueue of dgr_forward, in the reference's argument order, with capacity R_cap and the depth-range hint
+    (lo, hi), and no re-run when a frame overflows: (color, radii, workspace)."""
+    rs = GaussianRasterizationSettings(H, W, tan_fovx, tan_fovy, bg, scale_modifier, viewmatrix, projmatrix, degree,
+                                       campos, prefiltered, False)
+    color, radii, ws, _, _ = _forward(False, rs, means3D, sh, colors, opacity, scales, rotations, cov3D_precomp,
+                                      attempt=(R_cap, notify, lo, hi))
     return color, radii, ws
 
 
@@ -291,118 +394,12 @@ class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 raster_settings):
-        return _RasterizeGaussians._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                        cov3Ds_precomp, raster_settings)
+        return _fwd(ctx, False, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                    raster_settings)
 
     @staticmethod
     def backward(ctx, grad_out_color, _):
-        return _RasterizeGaussians._bwd(ctx, grad_out_color)   # its last entry, dL/dnormals, is None here
-
-    @staticmethod
-    def _fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-             raster_settings, maps=None, nrm=None, surf=None, cams=None, saved=()):
-        """maps: None (colour only) or the (depth, alpha) [1,H,W] tensors the forward writes as well.
-        nrm: None, or (normals [P,3], normal map [3,H,W]) for the normal map (with maps).
-        surf: None, or (near, far, median [1,H,W], distortion [1,H,W]) for the surface maps (with maps).
-        cams: None (the settings' camera), or the (viewmatrix, projmatrix, campos) to use instead.
-        saved: more tensors to save for the backward, after (means3D, radii)."""
-        rs = raster_settings
-        if cams is not None:
-            rs = rs._replace(viewmatrix=cams[0].detach(), projmatrix=cams[1].detach(), campos=cams[2].detach())
-        means3D = _f32c(means3D, "means3D")
-        if means3D is None:
-            raise ValueError("means3D must have dimensions (num_points, 3)")
-        t = (_f32c(rs.bg, "bg"), _f32c(sh, "sh"), _f32c(colors_precomp, "colors_precomp"),
-             _f32c(opacities, "opacities"), _f32c(scales, "scales"), _f32c(rotations, "rotations"),
-             _f32c(cov3Ds_precomp, "cov3D_precomp"), _f32c(rs.viewmatrix, "viewmatrix"),
-             _f32c(rs.projmatrix, "projmatrix"), _f32c(rs.campos, "campos"))
-        bg, sh_, col, opac, sc, rot, cov, view, proj, campos = t
-        H, W = int(rs.image_height), int(rs.image_width)
-        dev_index = means3D.device.index
-        key = (dev_index, W, H)
-        first = []
-
-        def run(R_cap, notify, lo, hi, mt):
-            o = _raw_forward(bg, means3D, col, opac, sc, rot, rs.scale_modifier, cov, view, proj, rs.tanfovx,
-                             rs.tanfovy, H, W, sh_, rs.sh_degree, campos, rs.prefiltered, R_cap, notify, lo, hi,
-                             first[0] if first else None, mt, maps, nrm, surf)
-            if not first:
-                first.append(o[:2])
-            return o
-
-        (color, radii, ws), _ = _run_sized(run, key, means3D.shape[0], dev_index)
-        if rs.debug:
-            torch.cuda.current_stream().synchronize()   # the reference's debug mode checks after every kernel
-        ctx.raster_settings = rs
-        ctx.ws = ws
-        ctx.R_cap = ws.R_cap
-        ctx.tensors = t
-        ctx.has_m2d = means2D is not None
-        ctx.save_for_backward(means3D, radii, *saved)
-        ctx.mark_non_differentiable(radii)
-        return color, radii
-
-    @staticmethod
-    def _bwd(ctx, grad_out_color, grad_depth=None, grad_alpha=None, cam=None, nrm=None, surf=None, abs_out=None):
-        """grad_depth / grad_alpha: None, or the upstream gradients of the maps (None = unused by the loss).
-        cam: None, or the _CameraGrads the backward writes the camera (and intrinsics) gradients to.
-        nrm: None, or (upstream gradient of the normal map, whether dL/dnormals is needed).
-        surf: None, or (near, far, upstream gradients of the median-depth and distortion maps, each None when
-        unused, not both).
-        abs_out: None, or the [P,3] tensor the backward writes the absolute screen-space gradient to.
-        Returns the eight Gaussian inputs' gradients in the reference's order, then dL/dnormals [P,3] (or None)."""
-        rs = ctx.raster_settings
-        bg, sh, col, opac, sc, rot, cov, view, proj, campos = ctx.tensors
-        means3D, radii = ctx.saved_tensors[:2]
-        ws = ctx.ws
-        P = means3D.shape[0]
-        H, W = int(rs.image_height), int(rs.image_width)
-        M = int(sh.shape[1]) if sh is not None else 0
-        # all nine gradients in one allocation (each sub-buffer 16-byte aligned for vector stores):
-        # m2d[P,3] (conic: not materialised) opac[P] col[P,3] m3d[P,3] cov[P,6] scale[P,3] rot[P,4] sh[P,M,3]
-        offs, o = [], 0
-        for w in (3, 0, 1, 3, 3, 6, 3, 4, 3 * M):
-            offs.append(o)
-            o = (o + P * w + 3) // 4 * 4
-        flat = torch.empty((max(o, 1),), dtype=torch.float32, device=means3D.device)
-        base = flat.data_ptr()
-        ptrs = [base + 4 * x for x in offs]
-
-        def gview(i, *shape):     # one as_strided per gradient (slice + view cost twice as much on the host)
-            stride, n = [], 1
-            for d in reversed(shape):
-                stride.append(n)
-                n *= d
-            return flat.as_strided(shape, stride[::-1], offs[i])
-
-        if grad_out_color is None:    # a depth / alpha loss only
-            grad_out_color = torch.zeros((3, H, W), dtype=torch.float32, device=means3D.device)
-        dpix = _f32c(grad_out_color, "grad_out_color")
-        p = _dgm_lib.ptr
-        head = (P, rs.sh_degree, M, p(bg), W, H, p(means3D), p(sh), p(col), p(sc), float(rs.scale_modifier), p(rot),
-                p(cov), p(view), p(proj), p(campos), float(rs.tanfovx), float(rs.tanfovy), p(radii), ws.geom,
-                ws.binning, ws.R_cap, ws.img, p(dpix))
-        grads = (ptrs[0], None, ptrs[2], ptrs[3], ptrs[4], ptrs[5], ptrs[8] if M else None, ptrs[6], ptrs[7])
-        aux = nrm_args = surf_args = dnormals = None
-        if grad_depth is not None or grad_alpha is not None:
-            aux = (p(_f32c(grad_depth, "grad_depth")), p(_f32c(grad_alpha, "grad_alpha")))
-        if nrm is not None:
-            if nrm[1]:
-                dnormals = torch.empty((P, 3), dtype=torch.float32, device=means3D.device)
-            nrm_args = (p(_f32c(nrm[0], "grad_normal")), p(dnormals), ws.nrm.data_ptr())
-        if surf is not None:
-            surf_args = (float(surf[0]), float(surf[1]), p(_f32c(surf[2], "grad_median_depth")),
-                         p(_f32c(surf[3], "grad_distortion")), ws.surf.data_ptr())
-        _enqueue("dgr_backward", ((None, head), ("_aux", aux), (None, grads),
-                                  ("_cam", None if cam is None else cam.args()), ("_nrm", nrm_args),
-                                  ("_surf", surf_args), ("_abs", None if abs_out is None else (p(abs_out),)),
-                                  ("_intr", None if cam is None else cam.intr_args()),
-                                  (None, (_dgm_lib.stream_ptr(),))))
-        # same ordering as the reference (:143-153)
-        return (gview(4, P, 3), gview(0, P, 3) if ctx.has_m2d else None,
-                gview(8, P, M, 3) if sh is not None else None, gview(3, P, 3) if col is not None else None,
-                gview(2, P, 1), gview(6, P, 3) if sc is not None else None,
-                gview(7, P, 4) if rot is not None else None, gview(5, P, 6) if cov is not None else None, dnormals)
+        return _bwd(ctx, grad_out_color)   # its last entry, dL/dnormals, is None here
 
 
 class _CameraGrads:
@@ -439,37 +436,6 @@ class _CameraGrads:
 _N_STREAMS = int(os.environ.get("DGMESH_B200_STREAMS", "2"))
 
 
-class _BatchWorkspace:
-    """F per-frame workspaces + F status blocks in one allocation (see dgr_forward_batch)."""
-    __slots__ = ("buf", "geom", "binning", "img", "status", "gs", "bs", "is_", "R_cap", "F", "nrm", "nrm_stride",
-                 "surf", "surf_stride")
-
-    def __init__(self, F, P, W, H, R_cap, dev, normal=False, surface=False):
-        _, _, _, ga, ba, ia = _sizes(P, W, H, R_cap)
-        self.buf = torch.empty((F * (ga + ba + ia) + 32 * F,), dtype=torch.uint8, device=dev)
-        base = self.buf.data_ptr()
-        self.geom, self.binning, self.img = base, base + F * ga, base + F * (ga + ba)
-        self.status = base + F * (ga + ba + ia)
-        self.gs, self.bs, self.is_, self.R_cap, self.F = ga, ba, ia, R_cap, F
-        # F normal workspaces of a normal forward (strides multiple of 512 bytes)
-        self.nrm_stride = (_normal_ws_bytes(P, R_cap) + 511) // 512 * 512 if normal else 0
-        self.nrm = torch.empty((F * self.nrm_stride,), dtype=torch.uint8, device=dev) if normal else None
-        # F surface workspaces of a surface forward
-        self.surf_stride = (_surface_ws_bytes(W, H) + 511) // 512 * 512 if surface else 0
-        self.surf = torch.empty((F * self.surf_stride,), dtype=torch.uint8, device=dev) if surface else None
-
-    def status_tensor(self):
-        return self.buf[-32 * self.F:].view(torch.int32).view(self.F, 8)
-
-    def frame(self, f):
-        """The workspace of frame f as a single-frame `_Workspace`-like view (for export_state)."""
-        w = _Workspace.__new__(_Workspace)
-        w.buf, w.R_cap = self.buf, self.R_cap
-        w.geom, w.binning, w.img = self.geom + f * self.gs, self.binning + f * self.bs, self.img + f * self.is_
-        w.status = self.status + 32 * f
-        return w
-
-
 _stacked = {}   # camera tensors' (address, version) -> stacked copies: a training loop reuses its cameras
 
 
@@ -503,6 +469,119 @@ def _fovs(settings):
 
 
 _PF_MEANS, _PF_SCALES, _PF_ROTS, _PF_OPAC, _PF_COLOR, _PF_COV = 1, 2, 4, 8, 16, 32
+_PF_MEAN2D = 64     # the screen-space gradients of a batch, which are per frame whatever the inputs are
+
+# The gradient outputs of the backward entry points, in each one's argument order: (slot, floats per Gaussian (per SH
+# coefficient for dL_dsh), per-frame bit, whether the entry requires it).  The slot is the output's place in the one
+# gradient allocation.  An output the entry does not require is passed as NULL unless its input is given.  Like the
+# reference's, dgr_backward takes every output but dL_dconic (not materialised) and dL_dsh; the batch entry points
+# also skip dL_dcolor and dL_dcov3D when they are not returned.
+_M2D, _CONIC, _OPAC, _COL, _M3D, _COV, _SCALE, _ROT, _SH = range(9)
+_BWD_GRADS = ((_M2D, 3, 0, True), (_CONIC, 0, 0, False), (_OPAC, 1, _PF_OPAC, True), (_COL, 3, _PF_COLOR, True),
+              (_M3D, 3, _PF_MEANS, True), (_COV, 6, _PF_COV, True), (_SH, 3, _PF_COLOR, False),
+              (_SCALE, 3, _PF_SCALES, True), (_ROT, 4, _PF_ROTS, True))
+_BWD_BATCH_GRADS = ((_M2D, 3, _PF_MEAN2D, True), (_OPAC, 1, _PF_OPAC, True), (_COL, 3, _PF_COLOR, False),
+                    (_M3D, 3, _PF_MEANS, True), (_COV, 6, _PF_COV, False), (_SH, 3, _PF_COLOR, False),
+                    (_SCALE, 3, _PF_SCALES, True), (_ROT, 4, _PF_ROTS, True))
+_REFERENCE_ORDER = (_M3D, _M2D, _SH, _COL, _OPAC, _SCALE, _ROT, _COV)     # the reference's gradient tuple (:143-153)
+
+
+def _fwd(ctx, batch, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings,
+         maps=None, nrm=None, surf=None, cams=None, saved=()):
+    """Forward of the rasterizer Functions: `_forward`, and what the backward needs kept in ctx.  saved: more
+    tensors to save for the backward, after (means3D, radii)."""
+    color, radii, ws, _, (means3D, ctx.tensors, ctx.fovs, ctx.pf) = _forward(
+        batch, settings, means3D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, maps, nrm, surf,
+        cams)
+    if not batch and settings.debug:
+        torch.cuda.current_stream().synchronize()   # the reference's debug mode checks after every kernel
+    ctx.raster_settings = settings[0] if batch else settings
+    ctx.ws = ws
+    ctx.has_m2d = means2D is not None
+    ctx.normals_pf = int(nrm is not None and nrm[0].ndim == 3)
+    ctx.save_for_backward(means3D, radii, *saved)
+    ctx.mark_non_differentiable(radii)
+    return color, radii
+
+
+def _grads(table, given, frames, F, P, M, dev):
+    """The gradient outputs of `table` (_BWD_GRADS) in one allocation, each sub-buffer 16-byte aligned for vector
+    stores: the outputs the entry requires or whose input is `given` (by slot), with F slabs where `frames` has
+    their per-frame bit.  Returns (their pointers in argument order, NULL where there is none, the gradient of each
+    given slot as a view, None elsewhere)."""
+    offs, o = [None] * 9, 0
+    for slot, w, bit, required in sorted(table):    # the sub-buffers in slot order
+        if required or given[slot]:
+            offs[slot] = o
+            o = (o + P * w * (M if slot == _SH else 1) * (F if frames & bit else 1) + 3) // 4 * 4
+    flat = torch.empty((max(o, 1),), dtype=torch.float32, device=dev)
+    base = flat.data_ptr()
+    ptrs = tuple([None if offs[slot] is None else base + 4 * offs[slot] for slot, _, _, _ in table])
+    views = [None] * 9
+    for slot, w, bit, _ in table:
+        if given[slot]:     # one as_strided per gradient (slice + view cost twice as much on the host)
+            shape, stride = ((P, M, 3), (3 * M, 3, 1)) if slot == _SH else ((P, w), (w, 1))
+            if frames & bit:
+                shape, stride = (F,) + shape, (P * stride[0],) + stride
+            views[slot] = flat.as_strided(shape, stride, offs[slot])
+    return ptrs, views
+
+
+def _bwd(ctx, grad_out_color, grad_depth=None, grad_alpha=None, cam=None, nrm=None, surf=None, abs_out=None):
+    """Backward of the rasterizer Functions through dgr_backward or dgr_backward_batch, the narrowest variant that
+    takes every segment in use (`_enqueue`).  The upstream gradients are shaped as the forward's outputs.
+    grad_depth / grad_alpha: None, or the upstream gradients of the maps (None = unused by the loss).
+    cam: None, or the _CameraGrads the backward writes the camera (and intrinsics) gradients to.
+    nrm: None, or (upstream gradient of the normal map, whether dL/dnormals is needed).
+    surf: None, or (near, far, upstream gradients of the median-depth and distortion maps, each None when unused, not
+    both).
+    abs_out: None, or the [P,3] ([F,P,3] for a batch) tensor the backward writes the absolute screen-space gradient to.
+    Returns the eight Gaussian inputs' gradients in the reference's order (a per-frame input's with a leading F),
+    then dL/dnormals [P,3] ([F,P,3] for per-frame normals), or None."""
+    rs = ctx.raster_settings
+    bg, sh, col, opac, sc, rot, cov, view, proj, campos = ctx.tensors
+    tx, ty = ctx.fovs
+    means3D, radii = ctx.saved_tensors[:2]
+    ws, pf, npf = ctx.ws, ctx.pf, ctx.normals_pf
+    batch, F, P, dev = bool(ws.lead), ws.F, means3D.shape[-2], means3D.device
+    H, W = int(rs.image_height), int(rs.image_width)
+    M = int(sh.shape[-2]) if sh is not None else 0
+    given = (ctx.has_m2d, False, True, col is not None, True, cov is not None, sc is not None, rot is not None,
+             sh is not None)    # by slot: means2D, conic, opacities, colours, means3D, cov3D, scales, rotations, SH
+    grads, views = _grads(_BWD_BATCH_GRADS if batch else _BWD_GRADS, given, (pf | _PF_MEAN2D) if batch else 0, F, P,
+                          M, dev)
+    if grad_out_color is None:    # a depth / alpha loss only
+        grad_out_color = torch.zeros(ws.lead + (3, H, W), dtype=torch.float32, device=dev)
+    dpix = _f32c(grad_out_color, "grad_out_color")
+    p = _dgm_lib.ptr
+    aux = gn = surf_args = dnormals = None
+    if grad_depth is not None or grad_alpha is not None:
+        aux = (p(_f32c(grad_depth, "grad_depth")), p(_f32c(grad_alpha, "grad_alpha")))
+    if nrm is not None:
+        if nrm[1]:
+            dnormals = torch.empty((F, P, 3) if npf else (P, 3), dtype=torch.float32, device=dev)
+        gn = p(_f32c(nrm[0], "grad_normal"))
+    if surf is not None:
+        surf_args = (float(surf[0]), float(surf[1]), p(_f32c(surf[2], "grad_median_depth")),
+                     p(_f32c(surf[3], "grad_distortion")), ws.surf.data_ptr())
+    if batch:
+        head = (F, P, rs.sh_degree, M, p(bg), W, H, p(means3D), p(sh), p(col), p(sc), float(rs.scale_modifier),
+                p(rot), p(cov), pf, p(view), p(proj), p(campos), tx, ty, p(radii), ws.geom, ws.gs, ws.binning, ws.bs,
+                ws.R_cap, ws.img, ws.is_, p(dpix))
+        tail = (_N_STREAMS, _dgm_lib.stream_ptr())
+        nrm_args = None if nrm is None else (gn, npf, p(dnormals), ws.nrm.data_ptr(), ws.nrm_stride)
+        surf_args = None if surf is None else surf_args + (ws.surf_stride,)
+    else:
+        head = (P, rs.sh_degree, M, p(bg), W, H, p(means3D), p(sh), p(col), p(sc), float(rs.scale_modifier), p(rot),
+                p(cov), p(view), p(proj), p(campos), float(tx), float(ty), p(radii), ws.geom, ws.binning, ws.R_cap,
+                ws.img, p(dpix))
+        tail = (_dgm_lib.stream_ptr(),)
+        nrm_args = None if nrm is None else (gn, p(dnormals), ws.nrm.data_ptr())
+    _enqueue("dgr_backward_batch" if batch else "dgr_backward", (
+        (None, head), ("_aux", aux), (None, grads), ("_cam", None if cam is None else cam.args()), ("_nrm", nrm_args),
+        ("_surf", surf_args), ("_abs", None if abs_out is None else (p(abs_out),)),
+        ("_intr", None if cam is None else cam.intr_args()), (None, tail)))
+    return tuple([views[slot] for slot in _REFERENCE_ORDER]) + (dnormals,)
 
 
 class _RasterizeGaussiansBatch(torch.autograd.Function):
@@ -516,160 +595,12 @@ class _RasterizeGaussiansBatch(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings):
-        return _RasterizeGaussiansBatch._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
-                                             cov3Ds_precomp, settings)
+        return _fwd(ctx, True, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                    settings)
 
     @staticmethod
     def backward(ctx, grad_out_color, _):
-        return _RasterizeGaussiansBatch._bwd(ctx, grad_out_color)   # its last entry, dL/dnormals, is None here
-
-    @staticmethod
-    def _fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings,
-             maps=None, nrm=None, surf=None, cams=None, saved=()):
-        """maps: None (colour only) or the (depth, alpha) [F,1,H,W] tensors the forward writes as well.
-        nrm: None, or (normals [P,3] shared or [F,P,3] per frame, normal maps [F,3,H,W]) (with maps).
-        surf: None, or (near, far, median [F,1,H,W], distortion [F,1,H,W]) (with maps).
-        cams: None (the settings' cameras), or the stacked (views [F,4,4], projs [F,4,4], campos [F,3]) to use.
-        saved: more tensors to save for the backward, after (means3D, radii)."""
-        rs0 = settings[0]
-        F = len(settings)
-        if F > _MAX_FRAMES:
-            raise ValueError(f"at most {_MAX_FRAMES} frames per batch")
-        for s in settings:
-            if (s.image_height, s.image_width, s.sh_degree, s.scale_modifier) != \
-                    (rs0.image_height, rs0.image_width, rs0.sh_degree, rs0.scale_modifier):
-                raise ValueError("all frames of a batch must share image size, SH degree and scale modifier")
-        means3D = _f32c(means3D, "means3D")
-        if means3D is None:
-            raise ValueError("means3D must have dimensions (num_points, 3)")
-        t = (_f32c(rs0.bg, "bg"), _f32c(sh, "sh"), _f32c(colors_precomp, "colors_precomp"),
-             _f32c(opacities, "opacities"), _f32c(scales, "scales"), _f32c(rotations, "rotations"),
-             _f32c(cov3Ds_precomp, "cov3D_precomp"))
-        bg, sh_, col, opac, sc, rot, cov = t
-        # per-frame mask from the ranks: means [F,P,3], scales [F,P,3], rotations [F,P,4], opacities [F,P,1],
-        # shs [F,P,M,3] / colors [F,P,3], cov3D [F,P,6]
-        pf = 0
-        for x, rank, bit in ((means3D, 3, _PF_MEANS), (sc, 3, _PF_SCALES), (rot, 3, _PF_ROTS), (opac, 3, _PF_OPAC),
-                             (sh_, 4, _PF_COLOR), (col, 3, _PF_COLOR), (cov, 3, _PF_COV)):
-            if x is not None and x.ndim == rank:
-                if x.shape[0] != F:
-                    raise ValueError("per-frame inputs must have a leading dimension equal to the number of frames")
-                pf |= bit
-        P = means3D.shape[-2]
-        if means3D.shape[-1] != 3:
-            raise ValueError("means3D must have dimensions (num_points, 3)")
-        dev = means3D.device
-        if cams is None:
-            views, projs, cams, tx, ty = _stack_settings(settings, dev)
-        else:
-            views, projs, cams = (_f32c(t.detach(), n) for t, n in zip(cams, ("viewmatrix", "projmatrix", "campos")))
-            tx, ty = _fovs(settings)
-        H, W = int(rs0.image_height), int(rs0.image_width)
-        M = int(sh_.shape[-2]) if sh_ is not None else 0
-        key = (dev.index, W, H)
-        p = _dgm_lib.ptr
-        first = []
-
-        def run(R_cap, notify, lo, hi, mt):
-            ws = _BatchWorkspace(F, P, W, H, R_cap, dev, nrm is not None, surf is not None)
-            if first:
-                color, radii = first[0]
-            else:
-                color = torch.empty((F, 3, H, W), dtype=torch.float32, device=dev)
-                radii = torch.empty((F, P), dtype=torch.int32, device=dev)
-                first.append((color, radii))
-            head = (F, P, rs0.sh_degree, M, p(bg), W, H, p(means3D), p(sh_), p(col), p(opac), p(sc),
-                    float(rs0.scale_modifier), p(rot), p(cov), pf, p(views), p(projs), p(cams), tx, ty,
-                    int(bool(rs0.prefiltered)), p(color), p(radii))
-            tail = (ws.geom, ws.gs, ws.binning, ws.bs, R_cap, ws.img, ws.is_, ws.status,
-                    notify.host_ptr if notify else None, notify.event if notify else None, lo, hi, int(mt),
-                    _N_STREAMS, _dgm_lib.stream_ptr())
-            _enqueue("dgr_forward_batch", (
-                (None, head), ("_aux", None if maps is None else (p(maps[0]), p(maps[1]))),
-                ("_nrm", None if nrm is None else (p(nrm[0]), int(nrm[0].ndim == 3), p(nrm[1]), ws.nrm.data_ptr(),
-                                                   ws.nrm_stride)),
-                ("_surf", None if surf is None else (float(surf[0]), float(surf[1]), p(surf[2]), p(surf[3]),
-                                                     ws.surf.data_ptr(), ws.surf_stride)),
-                (None, tail)))
-            return color, radii, ws
-
-        (color, radii, ws), _ = _run_sized(run, key, P, dev.index, F)
-        ctx.ws, ctx.tensors, ctx.cams, ctx.settings = ws, t, (views, projs, cams, tx, ty), settings
-        ctx.has_m2d = means2D is not None
-        ctx.pf = pf
-        ctx.normals_pf = int(nrm is not None and nrm[0].ndim == 3)
-        ctx.save_for_backward(means3D, radii, *saved)
-        ctx.mark_non_differentiable(radii)
-        return color, radii
-
-    @staticmethod
-    def _bwd(ctx, grad_out_color, grad_depth=None, grad_alpha=None, cam=None, nrm=None, surf=None, abs_out=None):
-        """As _RasterizeGaussians._bwd for F frames: the upstream gradients have a leading F dimension, abs_out is
-        [F,P,3], and dL/dnormals is [F,P,3] for per-frame normals, else [P,3]."""
-        bg, sh, col, opac, sc, rot, cov = ctx.tensors
-        views, projs, cams, tx, ty = ctx.cams
-        means3D, radii = ctx.saved_tensors[:2]
-        ws, rs0, pf = ctx.ws, ctx.settings[0], ctx.pf
-        F, P = ws.F, means3D.shape[-2]
-        H, W = int(rs0.image_height), int(rs0.image_width)
-        M = int(sh.shape[-2]) if sh is not None else 0
-
-        def nf(bit):
-            return F if (pf & bit) else 1
-
-        # m2d[F,P,3] opac col m3d cov scale rot sh -- per-frame inputs get F slabs; the colour gradient (with SH
-        # colours) and the cov3D gradient (without cov3D_precomp) are not returned, so they are not computed
-        widths = (3 * F, nf(_PF_OPAC), 3 * nf(_PF_COLOR) if col is not None else 0, 3 * nf(_PF_MEANS),
-                  6 * nf(_PF_COV) if cov is not None else 0, 3 * nf(_PF_SCALES), 4 * nf(_PF_ROTS),
-                  3 * M * nf(_PF_COLOR))
-        offs, o = [], 0
-        for w in widths:
-            offs.append(o)
-            o = (o + P * w + 3) // 4 * 4
-        flat = torch.empty((max(o, 1),), dtype=torch.float32, device=means3D.device)
-        base = flat.data_ptr()
-        ptrs = [base + 4 * x for x in offs]
-
-        def gview(i, bit, *shape):
-            if bit and (pf & bit):
-                shape = (F,) + shape
-            stride, n = [], 1
-            for d in reversed(shape):
-                stride.append(n)
-                n *= d
-            return flat.as_strided(shape, stride[::-1], offs[i])
-
-        if grad_out_color is None:    # a depth / alpha loss only
-            grad_out_color = torch.zeros((F, 3, H, W), dtype=torch.float32, device=means3D.device)
-        dpix = _f32c(grad_out_color, "grad_out_color")
-        p = _dgm_lib.ptr
-        head = (F, P, rs0.sh_degree, M, p(bg), W, H, p(means3D), p(sh), p(col), p(sc), float(rs0.scale_modifier),
-                p(rot), p(cov), pf, p(views), p(projs), p(cams), tx, ty, p(radii), ws.geom, ws.gs, ws.binning, ws.bs,
-                ws.R_cap, ws.img, ws.is_, p(dpix))
-        grads = (ptrs[0], ptrs[1], ptrs[2] if col is not None else None, ptrs[3], ptrs[4] if cov is not None else None,
-                 ptrs[7] if M else None, ptrs[5], ptrs[6])
-        aux = nrm_args = surf_args = dnormals = None
-        if grad_depth is not None or grad_alpha is not None:
-            aux = (p(_f32c(grad_depth, "grad_depth")), p(_f32c(grad_alpha, "grad_alpha")))
-        if nrm is not None:
-            npf = ctx.normals_pf
-            if nrm[1]:
-                dnormals = torch.empty((F, P, 3) if npf else (P, 3), dtype=torch.float32, device=means3D.device)
-            nrm_args = (p(_f32c(nrm[0], "grad_normal")), npf, p(dnormals), ws.nrm.data_ptr(), ws.nrm_stride)
-        if surf is not None:
-            surf_args = (float(surf[0]), float(surf[1]), p(_f32c(surf[2], "grad_median_depth")),
-                         p(_f32c(surf[3], "grad_distortion")), ws.surf.data_ptr(), ws.surf_stride)
-        _enqueue("dgr_backward_batch", ((None, head), ("_aux", aux), (None, grads),
-                                        ("_cam", None if cam is None else cam.args()), ("_nrm", nrm_args),
-                                        ("_surf", surf_args), ("_abs", None if abs_out is None else (p(abs_out),)),
-                                        ("_intr", None if cam is None else cam.intr_args()),
-                                        (None, (_N_STREAMS, _dgm_lib.stream_ptr()))))
-        return (gview(3, _PF_MEANS, P, 3), gview(0, 0, F, P, 3) if ctx.has_m2d else None,
-                gview(7, _PF_COLOR, P, M, 3) if sh is not None else None,
-                gview(2, _PF_COLOR, P, 3) if col is not None else None,
-                gview(1, _PF_OPAC, P, 1), gview(5, _PF_SCALES, P, 3) if sc is not None else None,
-                gview(6, _PF_ROTS, P, 4) if rot is not None else None,
-                gview(4, _PF_COV, P, 6) if cov is not None else None, dnormals)
+        return _bwd(ctx, grad_out_color)   # its last entry, dL/dnormals, is None here
 
 
 _MAX_FEATURES = 64
@@ -700,18 +631,11 @@ class _FeatureState:
         self.buf = torch.empty((max(n.value, 16),), dtype=torch.uint8, device=dev)
 
 
-def _ws_args(ws):
-    """(geom, stride, binning, stride, R_cap, img, stride) of a single-frame or batch workspace."""
-    if isinstance(ws, _BatchWorkspace):
-        return ws.geom, ws.gs, ws.binning, ws.bs, ws.R_cap, ws.img, ws.is_
-    return ws.geom, 0, ws.binning, 0, ws.R_cap, ws.img, 0
-
-
 def _features_fwd(ws, st, W, H, fmap):
     """dgr_features_fwd over the blend of the forward that wrote `ws`: fmap [F,C,H,W] (or [C,H,W])."""
     P = st.feats.shape[-2]
     _dgm_lib.check(_dgm_lib.lib().dgr_features_fwd(st.F, P, st.C, W, H, st.feats.data_ptr(), st.per_frame,
-                                                   *_ws_args(ws), fmap.data_ptr(), st.buf.data_ptr(), st.buf.numel(),
+                                                   *ws.side_args(), fmap.data_ptr(), st.buf.data_ptr(), st.buf.numel(),
                                                    _dgm_lib.stream_ptr()), "dgr_features_fwd")
 
 
@@ -722,7 +646,7 @@ def _features_bwd(ws, st, W, H, fmap, grad, need):
     g = _f32c(grad, "grad_features")
     dfeat = torch.empty(st.feats.shape, dtype=torch.float32, device=st.feats.device) if need else None
     _dgm_lib.check(_dgm_lib.lib().dgr_features_bwd(st.F, P, st.C, W, H, st.feats.data_ptr(), st.per_frame,
-                                                   *_ws_args(ws), fmap.data_ptr(), g.data_ptr(), _dgm_lib.ptr(dfeat),
+                                                   *ws.side_args(), fmap.data_ptr(), g.data_ptr(), _dgm_lib.ptr(dfeat),
                                                    st.buf.data_ptr(), st.buf.numel(), _dgm_lib.stream_ptr()),
                    "dgr_features_bwd")
     return dfeat
@@ -746,7 +670,7 @@ def _blend_stats(ws, P, W, H, F, weights):
     shape = (P,) if F is None else (F, P)
     out_sum, out_max = (torch.empty(shape, dtype=torch.float32, device=ws.buf.device) for _ in range(2))
     w, per_frame = (None, 0) if weights is None else weights
-    _, _, binning, bs, R_cap, img, is_ = _ws_args(ws)
+    _, _, binning, bs, R_cap, img, is_ = ws.side_args()
     _dgm_lib.check(_dgm_lib.lib().dgr_blend_stats(F or 1, P, W, H, binning, bs, R_cap, img, is_, _dgm_lib.ptr(w),
                                                   per_frame, out_sum.data_ptr(), out_max.data_ptr(),
                                                   _dgm_lib.stream_ptr()), "dgr_blend_stats")
@@ -898,14 +822,13 @@ def _maps_forward(ctx, batch, means3D, means2D, sh, colors_precomp, opacities, s
         pst = _PlanarState(_check_planes(planes, P, F), F or 1, W, H, dev)
         pmaps = (new_map(1), new_map(1))
     cams = None if viewmatrix is None else (viewmatrix, projmatrix, campos)
-    core = _RasterizeGaussiansBatch if batch else _RasterizeGaussians
     saved = (() if fmap is None else (fmap,)) + (() if pmaps is None else (pmaps[0],))
-    color, radii = core._fwd(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                             settings, maps, nrm, surf, cams, saved)
+    color, radii = _fwd(ctx, batch, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                        settings, maps, nrm, surf, cams, saved)
     if st is not None:
         _features_fwd(ctx.ws, st, W, H, fmap)
     if pst is not None:
-        _dgm_lib.check(_dgm_lib.lib().dgr_planar_fwd(pst.F, P, W, H, pst.planes.data_ptr(), *_ws_args(ctx.ws),
+        _dgm_lib.check(_dgm_lib.lib().dgr_planar_fwd(pst.F, P, W, H, pst.planes.data_ptr(), *ctx.ws.side_args(),
                                                      pmaps[0].data_ptr(), pmaps[1].data_ptr(), pst.buf.data_ptr(),
                                                      pst.buf.numel(), _dgm_lib.stream_ptr()), "dgr_planar_fwd")
     bstats = (None, None)
@@ -918,10 +841,10 @@ def _maps_forward(ctx, batch, means3D, means2D, sh, colors_precomp, opacities, s
         (None if nrm is None else nrm[1], fmap) + bstats + (pmaps or (None, None))
 
 
-def _maps_backward(ctx, core, grad_color, _, grad_depth, grad_alpha, grad_median, grad_dist, grad_normal,
-                   grad_features, _bsum, _bmax, grad_pdepth, grad_pmedian):
+def _maps_backward(ctx, grad_color, _, grad_depth, grad_alpha, grad_median, grad_dist, grad_normal, grad_features,
+                   _bsum, _bmax, grad_pdepth, grad_pmedian):
     """Backward of the maps Functions: the feature and planar passes first (they add to the forward's accumulators),
-    then `core`'s rasterizer backward with the segments the upstream gradients use."""
+    then the rasterizer backward with the segments the upstream gradients use."""
     *_, need_normals, need_features, need_planes, need_view, need_proj, need_campos, need_tanfov, need_abs, _, _ = \
         ctx.needs_input_grad
     means3D = ctx.saved_tensors[0]
@@ -936,7 +859,7 @@ def _maps_backward(ctx, core, grad_color, _, grad_depth, grad_alpha, grad_median
         dplanes = torch.empty(pst.planes.shape, dtype=torch.float32, device=means3D.device) if need_planes else None
         p = _dgm_lib.ptr
         _dgm_lib.check(_dgm_lib.lib().dgr_planar_bwd(
-            pst.F, means3D.shape[-2], W, H, pst.planes.data_ptr(), *_ws_args(ctx.ws), pdepth.data_ptr(),
+            pst.F, means3D.shape[-2], W, H, pst.planes.data_ptr(), *ctx.ws.side_args(), pdepth.data_ptr(),
             p(_f32c(grad_pdepth, "grad_planar_depth")), p(_f32c(grad_pmedian, "grad_planar_median_depth")),
             p(dplanes), pst.buf.data_ptr(), pst.buf.numel(), _dgm_lib.stream_ptr()), "dgr_planar_bwd")
     need = (need_view, need_proj, need_campos, need_tanfov)
@@ -944,7 +867,7 @@ def _maps_backward(ctx, core, grad_color, _, grad_depth, grad_alpha, grad_median
     ab = torch.empty(ctx.abs_shape, dtype=torch.float32, device=means3D.device) if need_abs else None
     nrm = None if grad_normal is None else (grad_normal, need_normals)
     surf = None if grad_median is None and grad_dist is None else (*ctx.surface, grad_median, grad_dist)
-    g = core._bwd(ctx, grad_color, grad_depth, grad_alpha, cam, nrm, surf, ab)
+    g = _bwd(ctx, grad_color, grad_depth, grad_alpha, cam, nrm, surf, ab)
     return g + (dfeat, dplanes) + (cam.grads(ctx.cam_shapes) if cam else (None,) * 4) + (ab, None, None)
 
 
@@ -970,7 +893,7 @@ class _RasterizeGaussiansMaps(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *grads):
-        return _maps_backward(ctx, _RasterizeGaussians, *grads)
+        return _maps_backward(ctx, *grads)
 
 
 class _RasterizeGaussiansBatchMaps(torch.autograd.Function):
@@ -984,7 +907,7 @@ class _RasterizeGaussiansBatchMaps(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *grads):
-        return _maps_backward(ctx, _RasterizeGaussiansBatch, *grads)
+        return _maps_backward(ctx, *grads)
 
 
 def rasterize_gaussians_batch(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
@@ -1032,7 +955,8 @@ def _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp):
             ((scales is not None or rotations is not None) and cov3D_precomp is not None):
         raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
     e = torch.Tensor([])
-    return tuple(e if x is None else x for x in (shs, colors_precomp, scales, rotations, cov3D_precomp))
+    return (e if shs is None else shs, e if colors_precomp is None else colors_precomp, e if scales is None else scales,
+            e if rotations is None else rotations, e if cov3D_precomp is None else cov3D_precomp)
 
 
 def _host_fovs(settings, batch=False, grad=False):
@@ -1104,16 +1028,8 @@ class BatchGaussianRasterizer(nn.Module):
         if means2D_abs is not None:
             return tuple(self._maps(means3D, means2D, opacities, shs, colors_precomp, scales, rotations, cov3D_precomp,
                                     means2D_abs=means2D_abs).values())
-        if (shs is None) == (colors_precomp is None):
-            raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-        if ((scales is None or rotations is None) and cov3D_precomp is None) or \
-                ((scales is not None or rotations is not None) and cov3D_precomp is not None):
-            raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
-        e = torch.Tensor([])
-        return rasterize_gaussians_batch(means3D, means2D, e if shs is None else shs,
-                                         e if colors_precomp is None else colors_precomp, opacities,
-                                         e if scales is None else scales, e if rotations is None else rotations,
-                                         e if cov3D_precomp is None else cov3D_precomp,
+        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
+        return rasterize_gaussians_batch(means3D, means2D, sh, col, opacities, sc, rot, cov,
                                          _host_fovs(self.settings, True)[0])
 
     def _maps(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
@@ -1249,24 +1165,8 @@ class GaussianRasterizer(nn.Module):
     def forward(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
                 cov3D_precomp=None):
         raster_settings = _host_fovs(self.raster_settings)[0]
-        # same argument-exclusivity errors as the reference (:191-195)
-        if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
-            raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-        if ((scales is None or rotations is None) and cov3D_precomp is None) or \
-                ((scales is not None or rotations is not None) and cov3D_precomp is not None):
-            raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
-        if shs is None:
-            shs = torch.Tensor([])
-        if colors_precomp is None:
-            colors_precomp = torch.Tensor([])
-        if scales is None:
-            scales = torch.Tensor([])
-        if rotations is None:
-            rotations = torch.Tensor([])
-        if cov3D_precomp is None:
-            cov3D_precomp = torch.Tensor([])
-        return rasterize_gaussians(means3D, means2D, shs, colors_precomp, opacities, scales, rotations, cov3D_precomp,
-                                   raster_settings)
+        sh, col, sc, rot, cov = _exclusive_inputs(shs, colors_precomp, scales, rotations, cov3D_precomp)
+        return rasterize_gaussians(means3D, means2D, sh, col, opacities, sc, rot, cov, raster_settings)
 
     def _maps(self, means3D, means2D, opacities, shs=None, colors_precomp=None, scales=None, rotations=None,
               cov3D_precomp=None, depth_alpha=False, normals=None, surface=None, features=None, camera_grad=False,
@@ -1407,24 +1307,9 @@ class _CCompat:
     def rasterize_gaussians(bg, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                             viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degree,
                             campos, prefiltered, debug):
-        a = [_f32c(x, n) for x, n in ((bg, "bg"), (means3D, "means3D"), (colors, "colors"), (opacity, "opacity"),
-                                      (scales, "scales"), (rotations, "rotations"), (cov3D_precomp, "cov3D"),
-                                      (viewmatrix, "view"), (projmatrix, "proj"), (sh, "sh"), (campos, "campos"))]
-        bg_, m3, col, op, sc, ro, cov, view, proj, sh_, cam = a
-        if m3 is None:
-            raise ValueError("means3D must have dimensions (num_points, 3)")
-        key = (m3.device.index, int(image_width), int(image_height))
-        first = []
-
-        def run(R_cap, notify, lo, hi, mt):
-            o = _raw_forward(bg_, m3, col, op, sc, ro, scale_modifier, cov, view, proj, tan_fovx, tan_fovy,
-                             int(image_height), int(image_width), sh_, degree, cam, prefiltered, R_cap, notify, lo, hi,
-                             first[0] if first else None, mt)
-            if not first:
-                first.append(o[:2])
-            return o
-
-        (color, radii, ws), R = _run_sized(run, key, m3.shape[0], m3.device.index)
+        rs = GaussianRasterizationSettings(image_height, image_width, tan_fovx, tan_fovy, bg, scale_modifier,
+                                           viewmatrix, projmatrix, degree, campos, prefiltered, debug)
+        color, radii, ws, R, _ = _forward(False, rs, means3D, sh, colors, opacity, scales, rotations, cov3D_precomp)
         if R is None:       # stream capture: this entry point returns R as a Python int and cannot be captured
             raise _dgm_lib.DgmError("_C.rasterize_gaussians returns num_rendered to the host: not capturable")
         # the three opaque byte tensors (views of one allocation) carry everything backward needs;
