@@ -247,6 +247,19 @@ SIGNATURES.update({
     "dgdr_backward": (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, P, P, P, P, P, P, P, P, c_size_t, P]),
 })
 
+# HexPlane field: (F, N, S, C, res_host, R_t) + forward: box, x, t, planes_host, out / backward: box, x, t,
+# planes_host, grad_out, grad_x, grad_planes_host, ws, bytes; the regularisers (S, C, res_host, R_t, planes_host) +
+# forward: losses, ws, bytes / backward: grad_losses, grad_planes_host; + stream
+_HP_HEAD = [c_int, c_int, c_int, c_int, P, c_int]
+SIGNATURES.update({
+    "dghp_forward": (c_int, _HP_HEAD + [P, P, P, P, P, P]),
+    "dghp_backward_workspace": (c_int, _HP_HEAD + [ctypes.POINTER(c_size_t)]),
+    "dghp_backward": (c_int, _HP_HEAD + [P, P, P, P, P, P, P, P, c_size_t, P]),
+    "dghp_reg_workspace": (c_int, _HP_HEAD[2:] + [ctypes.POINTER(c_size_t)]),
+    "dghp_reg_forward": (c_int, _HP_HEAD[2:] + [P, P, P, c_size_t, P]),
+    "dghp_reg_backward": (c_int, _HP_HEAD[2:] + [P, P, P, P]),
+})
+
 KERNEL_NAMES = ["preprocess", "tile_scan", "scatter", "sort_pack", "render_fwd", "render_bwd", "preprocess_bwd",
                 "count", "normal_grad_finish", "median_grad", "feature_fwd", "feature_bwd", "feature_grad_finish",
                 "blend_stats"]

@@ -15,6 +15,7 @@
 #include "metrics_kernels.h"
 #include "mesh_distance_kernels.h"
 #include "deform_reg_kernels.h"
+#include "hexplane_kernels.h"
 #include "meshrast_kernels.h"
 #include "nvls_kernels.h"
 
@@ -1904,6 +1905,142 @@ int dgdr_backward(int F, int P, int K, const int32_t* index, const float* weight
   return check(dgm::launch_deform_reg_bwd(F, P, K, index, weight, inv_offsets, inv_pairs, xyz_a, rot_a, xyz_b, rot_b,
                                           grad_losses, grad_xyz_a, grad_rot_a, grad_xyz_b, grad_rot_b, ws,
                                           (cudaStream_t)stream));
+}
+
+// ---- HexPlane field and its regularisers.  Every argument is checked here, before any device work.
+namespace {
+int dghp_field(const char* fn, int S, int C, const int32_t* res_host, int R_t, dgm::HpField& f) {
+  char msg[200];
+  if (S < 1 || S > HP_MAX_S || (C != 16 && C != 32) || R_t < 2) {
+    snprintf(msg, sizeof(msg), "%s: bad size (1 <= S <= 4, C = 16 or 32, R_t >= 2)", fn);
+    return bad(msg);
+  }
+  if (!res_host) {
+    snprintf(msg, sizeof(msg), "%s: null pointer (res_host)", fn);
+    return bad(msg);
+  }
+  memset(&f, 0, sizeof(f));
+  f.S = S, f.C = C, f.Rt = R_t;
+  for (int s = 0; s < S; ++s) {
+    const int64_t R = res_host[s];
+    if (R < 2 || R * R * C > INT32_MAX || (int64_t)R_t * R * C > INT32_MAX) {
+      snprintf(msg, sizeof(msg), "%s: bad size (resolutions >= 2, R R C and R_t R C < 2^31)", fn);
+      return bad(msg);
+    }
+    f.R[s] = (int)R;
+  }
+  return DGM_OK;
+}
+
+int dghp_sizes(const char* fn, int F, int N, int S, int C) {
+  char msg[200];
+  if (F < 0 || N < 0 || 3 * (int64_t)S * N * (1 + (int64_t)F) > INT32_MAX || (int64_t)F * N * S * C > INT32_MAX) {
+    snprintf(msg, sizeof(msg), "%s: bad size (F, N >= 0, 3 S N (1 + F) and F N S C < 2^31)", fn);
+    return bad(msg);
+  }
+  return DGM_OK;
+}
+
+// the field's shape and, when planes_host is given, its 6 S plane pointers (none may be NULL)
+int dghp_args(const char* fn, int F, int N, int S, int C, const int32_t* res_host, int R_t,
+              const float* const* planes_host, dgm::HpField& f) {
+  int rc = dghp_field(fn, S, C, res_host, R_t, f);
+  if (rc == DGM_OK) rc = dghp_sizes(fn, F, N, S, C);
+  if (rc != DGM_OK || !planes_host) return rc;
+  for (int p = 0; p < HP_PLANES * S; ++p) {
+    if (!planes_host[p]) {
+      char msg[200];
+      snprintf(msg, sizeof(msg), "%s: null pointer (plane %d)", fn, p);
+      return bad(msg);
+    }
+    f.p[p] = planes_host[p];
+  }
+  return DGM_OK;
+}
+
+int dghp_grads(const char* fn, int S, float* const* grad_planes_host, dgm::HpGrads& g) {
+  char msg[200];
+  for (int p = 0; p < HP_PLANES * S; ++p) {
+    if (!grad_planes_host[p]) {
+      snprintf(msg, sizeof(msg), "%s: null pointer (plane gradient %d)", fn, p);
+      return bad(msg);
+    }
+    g.p[p] = grad_planes_host[p];
+  }
+  return DGM_OK;
+}
+}  // namespace
+
+int dghp_forward(int F, int N, int S, int C, const int32_t* res_host, int R_t, const float* box, const float* x,
+                 const float* t, const float* const* planes_host, float* out, void* stream) {
+  dgm::HpField f;
+  if (!planes_host) return bad("dghp_forward: null pointer");
+  const int rc = dghp_args("dghp_forward", F, N, S, C, res_host, R_t, planes_host, f);
+  if (rc != DGM_OK) return rc;
+  if (F == 0 || N == 0) return DGM_OK;
+  if (!box || !x || !t || !out) return bad("dghp_forward: null pointer");
+  return check(dgm::launch_hexplane_fwd(F, N, f, box, x, t, out, (cudaStream_t)stream));
+}
+
+int dghp_backward_workspace(int F, int N, int S, int C, const int32_t* res_host, int R_t, size_t* bytes) {
+  dgm::HpField f;
+  const int rc = dghp_args("dghp_backward_workspace", F, N, S, C, res_host, R_t, nullptr, f);
+  if (rc != DGM_OK) return rc;
+  if (!bytes) return bad("dghp_backward_workspace: null pointer");
+  const size_t E = dgm::hp_entries(F, N, S), cells = dgm::hp_cells(f);
+  dgm::HpWS::from(nullptr, E, cells, C, E ? dgm::hp_cub_bytes(E, cells) : 0, bytes);
+  return DGM_OK;
+}
+
+int dghp_backward(int F, int N, int S, int C, const int32_t* res_host, int R_t, const float* box, const float* x,
+                  const float* t, const float* const* planes_host, const float* grad_out, float* grad_x,
+                  float* const* grad_planes_host, void* ws, size_t ws_bytes, void* stream) {
+  dgm::HpField f;
+  dgm::HpGrads g;
+  if (!planes_host || !grad_planes_host) return bad("dghp_backward: null pointer");
+  int rc = dghp_args("dghp_backward", F, N, S, C, res_host, R_t, planes_host, f);
+  if (rc == DGM_OK) rc = dghp_grads("dghp_backward", S, grad_planes_host, g);
+  if (rc != DGM_OK) return rc;
+  if (F > 0 && N > 0) {
+    if (!box || !x || !t || !grad_out || !ws) return bad("dghp_backward: null pointer");
+    size_t need;
+    dghp_backward_workspace(F, N, S, C, res_host, R_t, &need);
+    if (ws_bytes < need) return dge_short("dghp_backward", ws_bytes, need);
+  }
+  return check(dgm::launch_hexplane_bwd(F, N, f, box, x, t, grad_out, grad_x, g, ws, (cudaStream_t)stream));
+}
+
+int dghp_reg_workspace(int S, int C, const int32_t* res_host, int R_t, size_t* bytes) {
+  dgm::HpField f;
+  const int rc = dghp_field("dghp_reg_workspace", S, C, res_host, R_t, f);
+  if (rc != DGM_OK) return rc;
+  if (!bytes) return bad("dghp_reg_workspace: null pointer");
+  *bytes = dgm::hp_reg_ws_bytes(f);
+  return DGM_OK;
+}
+
+int dghp_reg_forward(int S, int C, const int32_t* res_host, int R_t, const float* const* planes_host, float* losses,
+                     void* ws, size_t ws_bytes, void* stream) {
+  dgm::HpField f;
+  if (!planes_host) return bad("dghp_reg_forward: null pointer");
+  const int rc = dghp_args("dghp_reg_forward", 0, 0, S, C, res_host, R_t, planes_host, f);
+  if (rc != DGM_OK) return rc;
+  if (!losses || !ws) return bad("dghp_reg_forward: null pointer");
+  const size_t need = dgm::hp_reg_ws_bytes(f);
+  if (ws_bytes < need) return dge_short("dghp_reg_forward", ws_bytes, need);
+  return check(dgm::launch_hexplane_reg_fwd(f, losses, ws, (cudaStream_t)stream));
+}
+
+int dghp_reg_backward(int S, int C, const int32_t* res_host, int R_t, const float* const* planes_host,
+                      const float* grad_losses, float* const* grad_planes_host, void* stream) {
+  dgm::HpField f;
+  dgm::HpGrads g;
+  if (!planes_host || !grad_planes_host) return bad("dghp_reg_backward: null pointer");
+  int rc = dghp_args("dghp_reg_backward", 0, 0, S, C, res_host, R_t, planes_host, f);
+  if (rc == DGM_OK) rc = dghp_grads("dghp_reg_backward", S, grad_planes_host, g);
+  if (rc != DGM_OK) return rc;
+  if (!grad_losses) return bad("dghp_reg_backward: null pointer");
+  return check(dgm::launch_hexplane_reg_bwd(f, grad_losses, g, (cudaStream_t)stream));
 }
 
 // ---- early notification objects: an event + a device-mapped pinned status mirror.  These are the

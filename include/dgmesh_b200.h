@@ -1329,6 +1329,47 @@ int dgdr_backward(int F, int P, int K, const int32_t* index, const float* weight
                   const float* rot_b, const float* grad_losses, float* grad_xyz_a, float* grad_rot_a,
                   float* grad_xyz_b, float* grad_rot_b, void* ws, size_t ws_bytes, void* stream);
 
+/* ------------------------------------------------------------------------
+ * HexPlane / K-Planes space-time feature field (4D-GS).  Device pointers, except res_host [S] (the spatial
+ * resolution of each scale), planes_host and grad_planes_host [6 S] (host arrays of device pointers).  Nothing
+ * allocates or synchronises with the host.  DGM_E_BADARG before any device work for: S outside [1, 4], C not 16 or
+ * 32, a resolution below 2, R R C or R_t R C >= 2^31 for a plane, N < 0, F < 0, 3 S N (1 + F) >= 2^31,
+ * F N S C >= 2^31, or a NULL pointer; a workspace below its query: DGM_E_WORKSPACE.  F = 0 or N = 0 writes nothing
+ * (the backward zeroes the plane gradients).
+ *
+ * The field: x [N,3] canonical positions, t [F,N] times, box [6] = (lo xyz, hi xyz) device floats.  Plane (s, p),
+ * p over the pairs (a, b) = (x,y) (x,z) (x,t) (y,z) (y,t) (z,t), is planes_host[6 s + p], channels-last [R_b, R_a, C]
+ * with R_x = R_y = R_z = res_host[s] and R_t.  Each plane is sampled bilinearly as grid_sample(align_corners=True,
+ * padding_mode='border'): pixel coordinate (x - lo) (R - 1) / (hi - lo) along a spatial axis and t (R_t - 1) along
+ * time, clamped to [0, R - 1]; a indexes the columns (width), b the rows.
+ *   out[f, n, s C + c] = prod_p sample_{s,p}(f, n)[c]   (out [F,N,S C]; computed as (s0 s1 s3) (s2 s4 s5)).
+ * dghp_forward keeps nothing for the backward.
+ * dghp_backward: grad_out [F,N,S C] -> grad_x [N,3] (NULL: not computed) and every plane's gradient
+ *   (grad_planes_host, each written, not accumulated).  The coordinate gradient is torch's: 0 outside the box and
+ *   on its faces.  The plane gradients are gathered through a stable sort of the samples by bilinear cell, without
+ *   float atomics: bit-identical from run to run.  Workspace: dghp_backward_workspace (depends on F, N and the
+ *   planes' shapes).
+ * dghp_reg_forward: losses [3] = (tv, time_smooth, l1_time), each summed over its planes and the scales, for G
+ *   [R_b, R_a, C]:
+ *     tv          (spatial planes): mean_{i<R_b-1,j,c} (G[i+1,j,c] - G[i,j,c])^2 + mean_{i,j<R_a-1,c} (G[i,j+1,c] - G[i,j,c])^2
+ *     time_smooth (time planes):    mean_{i<R_t-2,j,c} (G[i+2,j,c] - 2 G[i+1,j,c] + G[i,j,c])^2   (0 when R_t = 2)
+ *     l1_time     (time planes):    mean |1 - G|
+ *   The partial sums are added in a fixed order (bit-identical from run to run).  Workspace: dghp_reg_workspace.
+ * dghp_reg_backward: grad_losses [3] (device) -> every plane's gradient (written, not accumulated); d|1 - G|/dG is 0
+ *   at G = 1.
+ * ------------------------------------------------------------------------ */
+int dghp_forward(int F, int N, int S, int C, const int32_t* res_host, int R_t, const float* box, const float* x,
+                 const float* t, const float* const* planes_host, float* out, void* stream);
+int dghp_backward_workspace(int F, int N, int S, int C, const int32_t* res_host, int R_t, size_t* bytes);
+int dghp_backward(int F, int N, int S, int C, const int32_t* res_host, int R_t, const float* box, const float* x,
+                  const float* t, const float* const* planes_host, const float* grad_out, float* grad_x,
+                  float* const* grad_planes_host, void* ws, size_t ws_bytes, void* stream);
+int dghp_reg_workspace(int S, int C, const int32_t* res_host, int R_t, size_t* bytes);
+int dghp_reg_forward(int S, int C, const int32_t* res_host, int R_t, const float* const* planes_host, float* losses,
+                     void* ws, size_t ws_bytes, void* stream);
+int dghp_reg_backward(int S, int C, const int32_t* res_host, int R_t, const float* const* planes_host,
+                      const float* grad_losses, float* const* grad_planes_host, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
