@@ -85,10 +85,17 @@ SIGNATURES = {
     "dgp_plan_destroy": (c_int, [P]),
     "dgp_forward": (c_int, [P, c_int, ctypes.c_double, P, P, c_int, P, P, P, c_size_t, P]),
     "dgp_backward": (c_int, [P, c_int, P, P, c_int, P, P, P, P, P, c_size_t, P]),
+    "dgp_batch_workspace_size": (c_int, [P, c_int, ctypes.POINTER(c_size_t)]),
+    "dgp_forward_batch": (c_int, [P, c_int, c_int, ctypes.c_double, P, P, c_int, P, P, P, c_size_t, P]),
+    "dgp_backward_batch": (c_int, [P, c_int, c_int, P, P, c_int, P, P, P, P, P, c_size_t, P]),
     "dgmc_workspace_size": (c_int, [c_int, ctypes.POINTER(c_size_t)]),
     "dgmc_count": (c_int, [c_int, P, c_float, P, c_size_t, P, P, P, P]),
     "dgmc_emit": (c_int, [c_int, P, c_float, P, c_size_t, P, P, c_int64, P, c_int64, P]),
     "dgmc_backward": (c_int, [c_int, c_int, P, c_float, P, P, P, P]),
+    "dgmc_workspace_size_batch": (c_int, [c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "dgmc_count_batch": (c_int, [c_int, c_int, P, c_float, P, c_size_t, P, P, P, P]),
+    "dgmc_emit_batch": (c_int, [c_int, c_int, P, c_float, P, c_size_t, P, P, c_int64, P, c_int64, P]),
+    "dgmc_backward_batch": (c_int, [c_int, c_int, P, P, c_float, P, P, P, P]),
     "dgl_gemm_ws_bytes": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
     "dgl_gemm_bf16": (c_int, [c_int, c_int, c_int, P, c_int, P, c_int, P, c_int, P, c_int, P, c_size_t, P]),
     "dgl_gemm_tn_bf16": (c_int, [c_int, c_int, c_int, P, c_int, P, c_int, P, c_int, c_int, P, c_size_t, P]),
@@ -108,6 +115,12 @@ SIGNATURES = {
     "dgmr_interpolate_bwd": (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, P]),
     "dgmr_antialias": (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, P]),
     "dgmr_antialias_bwd": (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, P, P, P]),
+    "dgmr_rasterize_batch": (c_int, [c_int, c_int, c_int, P, c_int, c_int, P, P, P, P, P]),
+    "dgmr_rasterize_bwd_batch": (c_int, [c_int, c_int, c_int, P, P, P, P, P, P]),
+    "dgmr_interpolate_batch": (c_int, [c_int, c_int, c_int, c_int, P, P, P, P, P]),
+    "dgmr_interpolate_bwd_batch": (c_int, [c_int, c_int, c_int, c_int, P, P, P, P, P, P, P]),
+    "dgmr_antialias_batch": (c_int, [c_int, c_int, c_int, c_int, P, P, P, P, P, P, P]),
+    "dgmr_antialias_bwd_batch": (c_int, [c_int, c_int, c_int, c_int, P, P, P, P, P, P, P, P, P]),
     "dgd_workspace_size": (c_int, [c_int, ctypes.POINTER(c_size_t)]),
     "dgd_plan": (c_int, [c_int, P, P, P, P, c_float, c_float, ctypes.c_double, ctypes.c_double, c_int, c_float, P,
                          c_size_t, P, P]),

@@ -1211,7 +1211,7 @@ int dgp_plan_create(int G, void** plan, size_t* ws_bytes) {
     strncpy(g_last_error, "dgp_plan_create: cuFFT plan creation failed", sizeof(g_last_error) - 1);
     return DGM_E_LAUNCH;
   }
-  if (ws_bytes) dgm::DpsrWS::from(nullptr, G, work, ws_bytes);
+  if (ws_bytes) dgm::DpsrWS::from(nullptr, G, work, 1, ws_bytes);
   return DGM_OK;
 }
 
@@ -1220,78 +1220,185 @@ int dgp_plan_destroy(void* plan) {
   return DGM_OK;
 }
 
-static int dgp_check(void* plan, size_t ws_bytes, void* ws) {
-  if (!plan || !ws) return bad("dpsr: null plan / workspace");
+int dgp_batch_workspace_size(void* plan, int B, size_t* bytes) {
+  if (!plan || !bytes) return bad("dgp_batch_workspace_size: null plan / bytes");
+  if (B < 1 || B > dgm::DPSR_MAX_BATCH) return bad("dgp_batch_workspace_size: B out of range (1 <= B <= 64)");
+  dgm::DpsrWS::from(nullptr, dgm::dpsr_plan_res(plan), dgm::dpsr_plan_work(plan), B, bytes);
+  return DGM_OK;
+}
+
+static int dgp_check(const char* fn, void* plan, int B, size_t ws_bytes, void* ws) {
+  char msg[160];
+  if (!plan || !ws) {
+    snprintf(msg, sizeof(msg), "%s: null plan / workspace", fn);
+    return bad(msg);
+  }
+  if (B < 1 || B > dgm::DPSR_MAX_BATCH) {
+    snprintf(msg, sizeof(msg), "%s: B out of range (1 <= B <= 64)", fn);
+    return bad(msg);
+  }
   size_t need;
-  dgm::DpsrWS::from(nullptr, dgm::dpsr_plan_res(plan), dgm::dpsr_plan_work(plan), &need);
+  dgm::DpsrWS::from(nullptr, dgm::dpsr_plan_res(plan), dgm::dpsr_plan_work(plan), B, &need);
   if (ws_bytes < need) {
-    strncpy(g_last_error, "dpsr: workspace too small", sizeof(g_last_error) - 1);
+    snprintf(g_last_error, sizeof(g_last_error), "%s: workspace too small", fn);
     return DGM_E_WORKSPACE;
   }
   return DGM_OK;
+}
+
+int dgp_forward_batch(void* plan, int B, int N, double sig, const float* V, const float* Nrm, int mode,
+                      const float* thres, float* out, void* ws, size_t ws_bytes, void* stream) {
+  int rc = dgp_check("dgp_forward_batch", plan, B, ws_bytes, ws);
+  if (rc != DGM_OK) return rc;
+  if (N < 0 || !out || (N > 0 && (!V || !Nrm)) || (mode && !thres)) return bad("dgp_forward_batch: bad argument");
+  return check(dgm::launch_dpsr_forward(plan, B, N, sig, V, Nrm, mode, thres, out, ws, (cudaStream_t)stream));
+}
+
+int dgp_backward_batch(void* plan, int B, int N, const float* V, const float* Nrm, int mode, const float* dL_dout,
+                       float* dV, float* dN, float* dthres, void* ws, size_t ws_bytes, void* stream) {
+  int rc = dgp_check("dgp_backward_batch", plan, B, ws_bytes, ws);
+  if (rc != DGM_OK) return rc;
+  if (N < 0 || !dL_dout || (N > 0 && (!V || !Nrm || !dV || !dN))) return bad("dgp_backward_batch: bad argument");
+  return check(dgm::launch_dpsr_backward(plan, B, N, V, Nrm, mode, dL_dout, dV, dN, dthres, ws,
+                                         (cudaStream_t)stream));
 }
 
 int dgp_forward(void* plan, int N, double sig, const float* V, const float* Nrm, int mode, const float* thres,
                 float* out, void* ws, size_t ws_bytes, void* stream) {
-  int rc = dgp_check(plan, ws_bytes, ws);
+  int rc = dgp_check("dpsr", plan, 1, ws_bytes, ws);
   if (rc != DGM_OK) return rc;
   if (N < 0 || !out || (N > 0 && (!V || !Nrm)) || (mode && !thres)) return bad("dgp_forward: bad argument");
-  return check(dgm::launch_dpsr_forward(plan, N, sig, V, Nrm, mode, thres, out, ws, (cudaStream_t)stream));
+  return check(dgm::launch_dpsr_forward(plan, 1, N, sig, V, Nrm, mode, thres, out, ws, (cudaStream_t)stream));
 }
 
 int dgp_backward(void* plan, int N, const float* V, const float* Nrm, int mode, const float* dL_dout, float* dV,
                  float* dN, float* dthres, void* ws, size_t ws_bytes, void* stream) {
-  int rc = dgp_check(plan, ws_bytes, ws);
+  int rc = dgp_check("dpsr", plan, 1, ws_bytes, ws);
   if (rc != DGM_OK) return rc;
   if (N < 0 || !dL_dout || (N > 0 && (!V || !Nrm || !dV || !dN))) return bad("dgp_backward: bad argument");
-  return check(dgm::launch_dpsr_backward(plan, N, V, Nrm, mode, dL_dout, dV, dN, dthres, ws, (cudaStream_t)stream));
+  return check(dgm::launch_dpsr_backward(plan, 1, N, V, Nrm, mode, dL_dout, dV, dN, dthres, ws, (cudaStream_t)stream));
 }
 
 int dgmc_workspace_size(int G, size_t* bytes) {
   if (G < 2 || G > 800 || !bytes) return bad("dgmc_workspace_size: bad argument (2 <= G <= 800)");
-  dgm::McWS::from(nullptr, G, bytes);
+  dgm::McWS::from(nullptr, G, 1, bytes);
   return DGM_OK;
 }
 
-static int dgmc_check(int G, const float* phi, void* ws, size_t ws_bytes) {
-  if (G < 2 || G > 800 || !phi || !ws) return bad("marching cubes: bad argument (2 <= G <= 800)");
+int dgmc_workspace_size_batch(int B, int G, size_t* bytes) {
+  if (B < 1 || B > dgm::MC_MAX_BATCH) return bad("dgmc_workspace_size_batch: B out of range (1 <= B <= 64)");
+  if (G < 2 || G > 800 || !bytes) return bad("dgmc_workspace_size_batch: bad argument (2 <= G <= 800)");
+  dgm::McWS::from(nullptr, G, B, bytes);
+  return DGM_OK;
+}
+
+static int dgmc_check(const char* fn, int B, int G, const float* phi, void* ws, size_t ws_bytes) {
+  char msg[160];
+  if (B < 1 || B > dgm::MC_MAX_BATCH) {
+    snprintf(msg, sizeof(msg), "%s: B out of range (1 <= B <= 64)", fn);
+    return bad(msg);
+  }
+  if (G < 2 || G > 800 || !phi || !ws) {
+    snprintf(msg, sizeof(msg), "%s: bad argument (2 <= G <= 800)", fn);
+    return bad(msg);
+  }
   size_t need;
-  dgm::McWS::from(nullptr, G, &need);
+  dgm::McWS::from(nullptr, G, B, &need);
   if (ws_bytes < need) {
-    strncpy(g_last_error, "marching cubes: workspace too small", sizeof(g_last_error) - 1);
+    snprintf(g_last_error, sizeof(g_last_error), "%s: workspace too small", fn);
     return DGM_E_WORKSPACE;
   }
   return DGM_OK;
 }
 
+static int dgmc_count_call(const char* fn, int B, int G, const float* phi, float iso, void* ws, size_t ws_bytes,
+                           int32_t* totals, int32_t* totals_host, void* totals_event, void* stream) {
+  int rc = dgmc_check(fn, B, G, phi, ws, ws_bytes);
+  if (rc != DGM_OK) return rc;
+  if (!totals) return bad(B == 1 ? "dgmc_count: null totals" : "dgmc_count_batch: null totals");
+  return check(dgm::launch_mc_count(B, G, phi, iso, ws, totals, totals_host, (cudaEvent_t)totals_event,
+                                    (cudaStream_t)stream));
+}
+
 int dgmc_count(int G, const float* phi, float iso, void* ws, size_t ws_bytes, int32_t* totals, int32_t* totals_host,
                void* totals_event, void* stream) {
-  int rc = dgmc_check(G, phi, ws, ws_bytes);
+  return dgmc_count_call("marching cubes", 1, G, phi, iso, ws, ws_bytes, totals, totals_host, totals_event, stream);
+}
+
+int dgmc_count_batch(int B, int G, const float* phi, float iso, void* ws, size_t ws_bytes, int32_t* totals,
+                     int32_t* totals_host, void* totals_event, void* stream) {
+  return dgmc_count_call("dgmc_count_batch", B, G, phi, iso, ws, ws_bytes, totals, totals_host, totals_event,
+                         stream);
+}
+
+static int dgmc_emit_call(const char* fn, int B, int G, const float* phi, float iso, void* ws, size_t ws_bytes,
+                          float* verts, int32_t* vsrc, int64_t V_cap, int32_t* faces, int64_t F_cap, void* stream) {
+  char msg[160];
+  // vertex indices are packed into 29 bits and face counts are int32: larger capacities could never be filled
+  if (V_cap < 0 || V_cap > dgm::MC_MAX_VERTS || F_cap < 0 || F_cap > INT32_MAX) {
+    snprintf(msg, sizeof(msg), "%s: capacity out of range (V_cap <= 2^29, F_cap < 2^31)", fn);
+    return bad(msg);
+  }
+  if ((V_cap > 0 && (!verts || !vsrc)) || (F_cap > 0 && !faces)) {
+    snprintf(msg, sizeof(msg), "%s: null output", fn);
+    return bad(msg);
+  }
+  int rc = dgmc_check(B == 1 ? "marching cubes" : fn, B, G, phi, ws, ws_bytes);
   if (rc != DGM_OK) return rc;
-  if (!totals) return bad("dgmc_count: null totals");
-  return check(dgm::launch_mc_count(G, phi, iso, ws, totals, totals_host, (cudaEvent_t)totals_event,
-                                    (cudaStream_t)stream));
+  return check(dgm::launch_mc_emit(B, G, phi, iso, ws, verts, vsrc, V_cap, faces, F_cap, (cudaStream_t)stream));
 }
 
 int dgmc_emit(int G, const float* phi, float iso, void* ws, size_t ws_bytes, float* verts, int32_t* vsrc,
               int64_t V_cap, int32_t* faces, int64_t F_cap, void* stream) {
-  // vertex indices are packed into 29 bits and face counts are int32: larger capacities could never be filled
-  if (V_cap < 0 || V_cap > dgm::MC_MAX_VERTS || F_cap < 0 || F_cap > INT32_MAX)
-    return bad("dgmc_emit: capacity out of range (V_cap <= 2^29, F_cap < 2^31)");
-  if ((V_cap > 0 && (!verts || !vsrc)) || (F_cap > 0 && !faces)) return bad("dgmc_emit: null output");
-  int rc = dgmc_check(G, phi, ws, ws_bytes);
-  if (rc != DGM_OK) return rc;
-  return check(dgm::launch_mc_emit(G, phi, iso, ws, verts, vsrc, V_cap, faces, F_cap, (cudaStream_t)stream));
+  return dgmc_emit_call("dgmc_emit", 1, G, phi, iso, ws, ws_bytes, verts, vsrc, V_cap, faces, F_cap, stream);
+}
+
+int dgmc_emit_batch(int B, int G, const float* phi, float iso, void* ws, size_t ws_bytes, float* verts,
+                    int32_t* vsrc, int64_t V_cap, int32_t* faces, int64_t F_cap, void* stream) {
+  return dgmc_emit_call("dgmc_emit_batch", B, G, phi, iso, ws, ws_bytes, verts, vsrc, V_cap, faces, F_cap, stream);
+}
+
+// V_host[B]: each item's vertex count (from dgmc_count / dgmc_count_batch)
+static int dgmc_backward_call(const char* fn, int B, int G, const int32_t* V_host, const float* phi, float iso,
+                              const int32_t* vsrc, const float* dL_dverts, float* dL_dphi, void* stream) {
+  char msg[160];
+  if (B < 1 || B > dgm::MC_MAX_BATCH) {
+    snprintf(msg, sizeof(msg), "%s: B out of range (1 <= B <= 64)", fn);
+    return bad(msg);
+  }
+  if (G < 2 || G > 800 || !phi || !dL_dphi || !V_host) {
+    snprintf(msg, sizeof(msg), "%s: bad argument (2 <= G <= 800)", fn);
+    return bad(msg);
+  }
+  // each V_k comes from dgmc_count: at most one vertex per grid edge; the batch within the 29-bit packing of dgmc_emit
+  const long long edges = 3ll * G * G * (G - 1);
+  dgm::McItems it;
+  it.B = B;
+  long long total = 0;
+  for (int k = 0; k < B; ++k) {
+    it.voff[k] = (int)total;
+    if (V_host[k] < 0 || V_host[k] > edges || total + V_host[k] > dgm::MC_MAX_VERTS) {
+      snprintf(msg, sizeof(msg), "%s: V out of range", fn);
+      return bad(msg);
+    }
+    total += V_host[k];
+  }
+  it.voff[B] = (int)total;
+  if (total > 0 && (!vsrc || !dL_dverts)) {
+    snprintf(msg, sizeof(msg), "%s: null vsrc / dL_dverts", fn);
+    return bad(msg);
+  }
+  return check(dgm::launch_mc_backward(G, it, phi, iso, vsrc, dL_dverts, dL_dphi, (cudaStream_t)stream));
 }
 
 int dgmc_backward(int G, int V, const float* phi, float iso, const int32_t* vsrc, const float* dL_dverts,
                   float* dL_dphi, void* stream) {
-  if (G < 2 || G > 800 || !phi || !dL_dphi) return bad("dgmc_backward: bad argument (2 <= G <= 800)");
-  // V comes from dgmc_count: at most one vertex per grid edge, and within the 29-bit packing of dgmc_emit
-  const long long edges = 3ll * G * G * (G - 1);
-  if (V < 0 || V > edges || V > dgm::MC_MAX_VERTS) return bad("dgmc_backward: V out of range");
-  if (V > 0 && (!vsrc || !dL_dverts)) return bad("dgmc_backward: null vsrc / dL_dverts");
-  return check(dgm::launch_mc_backward(G, V, phi, iso, vsrc, dL_dverts, dL_dphi, (cudaStream_t)stream));
+  return dgmc_backward_call("dgmc_backward", 1, G, &V, phi, iso, vsrc, dL_dverts, dL_dphi, stream);
+}
+
+int dgmc_backward_batch(int B, int G, const int32_t* V_host, const float* phi, float iso, const int32_t* vsrc,
+                        const float* dL_dverts, float* dL_dphi, void* stream) {
+  return dgmc_backward_call("dgmc_backward_batch", B, G, V_host, phi, iso, vsrc, dL_dverts, dL_dphi, stream);
 }
 
 int dgl_gemm_ws_bytes(int M, int N, int K, size_t* bytes) {
@@ -1446,40 +1553,172 @@ int dgl_laplacian_backward(int V, int F, const int32_t* tri, const float* dL_dlo
   return check(dgm::launch_laplacian_backward(V, F, tri, dL_dloss, dverts, ws, (cudaStream_t)stream));
 }
 
+// the B images of a call: 1 <= B <= 64, and for the rasteriser ranges[B][2] = (first triangle, count) within F
+static int dgmr_batch(const char* fn, int B) {
+  char msg[160];
+  if (B < 1 || B > dgm::MR_MAX_BATCH) {
+    snprintf(msg, sizeof(msg), "%s: B out of range (1 <= B <= 64)", fn);
+    return bad(msg);
+  }
+  return DGM_OK;
+}
+
+static int dgmr_ranges(int B, int F, const int32_t* ranges, dgm::MrRanges& R) {
+  int rc = dgmr_batch("dgmr_rasterize_batch", B);
+  if (rc != DGM_OK) return rc;
+  if (!ranges) return bad("dgmr_rasterize_batch: null ranges");
+  R.B = B;
+  long long total = 0;
+  for (int b = 0; b < B; ++b) {
+    const long long first = ranges[2 * b], count = ranges[2 * b + 1];
+    if (first < 0 || count < 0 || first + count > F)
+      return bad("dgmr_rasterize_batch: a range runs past F (0 <= first, 0 <= count, first + count <= F)");
+    R.start[b] = (int)first;
+    R.off[b] = (int)total;
+    total += count;
+    if (total > INT32_MAX) return bad("dgmr_rasterize_batch: more than 2^31 - 1 triangles in all ranges");
+  }
+  R.off[B] = (int)total;
+  return DGM_OK;
+}
+
+static int dgmr_rasterize_call(const char* fn, int V, int F, int W, int H, const float* pos, const int32_t* tri,
+                               void* zbuf, float* rast, const dgm::MrRanges& R, void* stream) {
+  char msg[160];
+  if (V < 0 || F < 0 || W <= 0 || H <= 0 || !zbuf || !rast || (F > 0 && (!pos || !tri))) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", fn);
+    return bad(msg);
+  }
+  if (F > dgm::MR_MAX_TRIANGLES) {
+    snprintf(msg, sizeof(msg), "%s: F beyond 2^29 triangles (the largest id rast holds)", fn);
+    return bad(msg);
+  }
+  return check(dgm::launch_mr_rasterize(R, W, H, pos, tri, zbuf, rast, (cudaStream_t)stream));
+}
+
 int dgmr_rasterize(int V, int F, int W, int H, const float* pos, const int32_t* tri, void* zbuf, float* rast,
                    void* stream) {
-  if (V < 0 || F < 0 || W <= 0 || H <= 0 || !zbuf || !rast || (F > 0 && (!pos || !tri)))
-    return bad("dgmr_rasterize: bad argument");
-  return check(dgm::launch_mr_rasterize(V, F, W, H, pos, tri, zbuf, rast, (cudaStream_t)stream));
+  dgm::MrRanges R;
+  R.B = 1;
+  R.start[0] = 0;
+  R.off[0] = 0;
+  R.off[1] = F > 0 ? F : 0;
+  return dgmr_rasterize_call("dgmr_rasterize", V, F, W, H, pos, tri, zbuf, rast, R, stream);
+}
+int dgmr_rasterize_batch(int V, int F, int B, const int32_t* ranges, int W, int H, const float* pos,
+                         const int32_t* tri, void* zbuf, float* rast, void* stream) {
+  dgm::MrRanges R;
+  int rc = dgmr_ranges(B, F, ranges, R);
+  if (rc != DGM_OK) return rc;
+  return dgmr_rasterize_call("dgmr_rasterize_batch", V, F, W, H, pos, tri, zbuf, rast, R, stream);
+}
+
+static int dgmr_rasterize_bwd_call(const char* fn, int B, int W, int H, const float* rast, const int32_t* tri,
+                                   const float* pos, const float* grast, float* gpos, void* stream) {
+  char msg[160];
+  int rc = dgmr_batch(fn, B);
+  if (rc != DGM_OK) return rc;
+  if (W <= 0 || H <= 0 || !rast || !tri || !pos || !grast || !gpos) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", fn);
+    return bad(msg);
+  }
+  return check(dgm::launch_mr_rasterize_bwd(B, W, H, rast, tri, pos, grast, gpos, (cudaStream_t)stream));
 }
 int dgmr_rasterize_bwd(int W, int H, const float* rast, const int32_t* tri, const float* pos, const float* grast,
                        float* gpos, void* stream) {
-  if (W <= 0 || H <= 0 || !rast || !tri || !pos || !grast || !gpos) return bad("dgmr_rasterize_bwd: bad argument");
-  return check(dgm::launch_mr_rasterize_bwd(W, H, rast, tri, pos, grast, gpos, (cudaStream_t)stream));
+  return dgmr_rasterize_bwd_call("dgmr_rasterize_bwd", 1, W, H, rast, tri, pos, grast, gpos, stream);
+}
+int dgmr_rasterize_bwd_batch(int B, int W, int H, const float* rast, const int32_t* tri, const float* pos,
+                             const float* grast, float* gpos, void* stream) {
+  return dgmr_rasterize_bwd_call("dgmr_rasterize_bwd_batch", B, W, H, rast, tri, pos, grast, gpos, stream);
+}
+
+static int dgmr_interpolate_call(const char* fn, int B, int W, int H, int C, const float* attr, const float* rast,
+                                 const int32_t* tri, float* out, void* stream) {
+  char msg[160];
+  int rc = dgmr_batch(fn, B);
+  if (rc != DGM_OK) return rc;
+  if (W <= 0 || H <= 0 || C < 1 || !attr || !rast || !tri || !out) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", fn);
+    return bad(msg);
+  }
+  return check(dgm::launch_mr_interpolate(B, W, H, C, attr, rast, tri, out, (cudaStream_t)stream));
 }
 int dgmr_interpolate(int W, int H, int C, const float* attr, const float* rast, const int32_t* tri, float* out,
                      void* stream) {
-  if (W <= 0 || H <= 0 || C < 1 || !attr || !rast || !tri || !out) return bad("dgmr_interpolate: bad argument");
-  return check(dgm::launch_mr_interpolate(W, H, C, attr, rast, tri, out, (cudaStream_t)stream));
+  return dgmr_interpolate_call("dgmr_interpolate", 1, W, H, C, attr, rast, tri, out, stream);
+}
+int dgmr_interpolate_batch(int B, int W, int H, int C, const float* attr, const float* rast, const int32_t* tri,
+                           float* out, void* stream) {
+  return dgmr_interpolate_call("dgmr_interpolate_batch", B, W, H, C, attr, rast, tri, out, stream);
+}
+
+static int dgmr_interpolate_bwd_call(const char* fn, int B, int W, int H, int C, const float* attr, const float* rast,
+                                     const int32_t* tri, const float* gout, float* gattr, float* grast,
+                                     void* stream) {
+  char msg[160];
+  int rc = dgmr_batch(fn, B);
+  if (rc != DGM_OK) return rc;
+  if (W <= 0 || H <= 0 || C < 1 || !attr || !rast || !tri || !gout) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", fn);
+    return bad(msg);
+  }
+  return check(dgm::launch_mr_interpolate_bwd(B, W, H, C, attr, rast, tri, gout, gattr, grast, (cudaStream_t)stream));
 }
 int dgmr_interpolate_bwd(int W, int H, int C, const float* attr, const float* rast, const int32_t* tri,
                          const float* gout, float* gattr, float* grast, void* stream) {
-  if (W <= 0 || H <= 0 || C < 1 || !attr || !rast || !tri || !gout) return bad("dgmr_interpolate_bwd: bad argument");
-  return check(dgm::launch_mr_interpolate_bwd(W, H, C, attr, rast, tri, gout, gattr, grast, (cudaStream_t)stream));
+  return dgmr_interpolate_bwd_call("dgmr_interpolate_bwd", 1, W, H, C, attr, rast, tri, gout, gattr, grast, stream);
+}
+int dgmr_interpolate_bwd_batch(int B, int W, int H, int C, const float* attr, const float* rast, const int32_t* tri,
+                               const float* gout, float* gattr, float* grast, void* stream) {
+  return dgmr_interpolate_bwd_call("dgmr_interpolate_bwd_batch", B, W, H, C, attr, rast, tri, gout, gattr, grast,
+                                   stream);
+}
+
+static int dgmr_antialias_call(const char* fn, int B, int W, int H, int C, const float* color, const float* rast,
+                               const float* pos, const int32_t* tri, const int32_t* opp, float* out, void* stream) {
+  char msg[160];
+  int rc = dgmr_batch(fn, B);
+  if (rc != DGM_OK) return rc;
+  if (W <= 0 || H <= 0 || C < 1 || !color || !rast || !pos || !tri || !opp || !out) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", fn);
+    return bad(msg);
+  }
+  return check(dgm::launch_mr_antialias(B, W, H, C, color, rast, pos, tri, opp, out, (cudaStream_t)stream));
 }
 int dgmr_antialias(int W, int H, int C, const float* color, const float* rast, const float* pos,
                    const int32_t* tri, const int32_t* opp, float* out, void* stream) {
-  if (W <= 0 || H <= 0 || C < 1 || !color || !rast || !pos || !tri || !opp || !out)
-    return bad("dgmr_antialias: bad argument");
-  return check(dgm::launch_mr_antialias(W, H, C, color, rast, pos, tri, opp, out, (cudaStream_t)stream));
+  return dgmr_antialias_call("dgmr_antialias", 1, W, H, C, color, rast, pos, tri, opp, out, stream);
+}
+int dgmr_antialias_batch(int B, int W, int H, int C, const float* color, const float* rast, const float* pos,
+                         const int32_t* tri, const int32_t* opp, float* out, void* stream) {
+  return dgmr_antialias_call("dgmr_antialias_batch", B, W, H, C, color, rast, pos, tri, opp, out, stream);
+}
+
+static int dgmr_antialias_bwd_call(const char* fn, int B, int W, int H, int C, const float* color, const float* rast,
+                                   const float* pos, const int32_t* tri, const int32_t* opp, const float* gout,
+                                   float* gcolor, float* gpos, void* stream) {
+  char msg[160];
+  int rc = dgmr_batch(fn, B);
+  if (rc != DGM_OK) return rc;
+  if (W <= 0 || H <= 0 || C < 1 || !color || !rast || !pos || !tri || !opp || !gout) {
+    snprintf(msg, sizeof(msg), "%s: bad argument", fn);
+    return bad(msg);
+  }
+  return check(dgm::launch_mr_antialias_bwd(B, W, H, C, color, rast, pos, tri, opp, gout, gcolor, gpos,
+                                            (cudaStream_t)stream));
 }
 int dgmr_antialias_bwd(int W, int H, int C, const float* color, const float* rast, const float* pos,
                        const int32_t* tri, const int32_t* opp, const float* gout, float* gcolor, float* gpos,
                        void* stream) {
-  if (W <= 0 || H <= 0 || C < 1 || !color || !rast || !pos || !tri || !opp || !gout)
-    return bad("dgmr_antialias_bwd: bad argument");
-  return check(dgm::launch_mr_antialias_bwd(W, H, C, color, rast, pos, tri, opp, gout, gcolor, gpos,
-                                            (cudaStream_t)stream));
+  return dgmr_antialias_bwd_call("dgmr_antialias_bwd", 1, W, H, C, color, rast, pos, tri, opp, gout, gcolor, gpos,
+                                 stream);
+}
+int dgmr_antialias_bwd_batch(int B, int W, int H, int C, const float* color, const float* rast, const float* pos,
+                             const int32_t* tri, const int32_t* opp, const float* gout, float* gcolor, float* gpos,
+                             void* stream) {
+  return dgmr_antialias_bwd_call("dgmr_antialias_bwd_batch", B, W, H, C, color, rast, pos, tri, opp, gout, gcolor,
+                                 gpos, stream);
 }
 
 int dgd_workspace_size(int P, size_t* bytes) {

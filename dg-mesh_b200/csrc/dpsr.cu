@@ -310,18 +310,20 @@ __global__ void __launch_bounds__(256) dpsr_bwd_points_kernel(int N, int G, floa
 }
 
 // ------------------------------------------------------------------ host side
-DpsrWS DpsrWS::from(char* base, int G, size_t fft_bytes, size_t* bytes) {
+// B items: phi_raw, red and scal are per item (item k at k * G^3, 4 k, 8 k) and outlive the forward; the rest is
+// scratch that the stages of one item use and the next item reuses.  B = 1 is the single-item layout.
+DpsrWS DpsrWS::from(char* base, int G, size_t fft_bytes, int B, size_t* bytes) {
   char* p = base;
   DpsrWS w;
   const size_t G3 = (size_t)G * G * G, Gs = (size_t)G * G * (G / 2 + 1);
   w.ras = carve<float>(p, 3 * G3);        // normals grid (fwd) / dras (bwd)
   w.spec = carve<float2>(p, 3 * Gs);      // spectra of the three channels
   w.phi_hat = carve<float2>(p, Gs);       // solved field, half spectrum
-  w.phi_raw = carve<float>(p, G3);        // unscaled C2R output (kept for the backward pass)
+  w.phi_raw = carve<float>(p, (size_t)B * G3);  // unscaled C2R output (kept for the backward pass)
   w.dphi = carve<float>(p, G3);
   w.lut = carve<float>(p, 3 * (size_t)(G / 2 + 1) * (G / 2 + 1) + 8);
-  w.red = carve<double>(p, 4);            // [0] sum of fv (fwd);  [1..2] A, B (bwd)
-  w.scal = carve<float>(p, 8);            // offset, fv0, coef
+  w.red = carve<double>(p, 4 * (size_t)B);  // [0] sum of fv (fwd);  [1..2] A, B (bwd)
+  w.scal = carve<float>(p, 8 * (size_t)B);  // offset, fv0, coef
   w.fft_work = carve<char>(p, fft_bytes);
   if (bytes) *bytes = size_t(p - base) + 128;
   return w;
@@ -373,53 +375,67 @@ static bool use(cufftHandle h, void* work, cudaStream_t s) {
   return cufftSetStream(h, s) == CUFFT_SUCCESS && cufftSetWorkArea(h, work) == CUFFT_SUCCESS;
 }
 
-cudaError_t launch_dpsr_forward(void* plan, int N, double sig, const float* V, const float* Nrm, int mode,
+// items are V[B,N,3], Nrm[B,N,3] -> out[B,G,G,G]; each item runs the whole chain on the shared scratch
+cudaError_t launch_dpsr_forward(void* plan, int B, int N, double sig, const float* V, const float* Nrm, int mode,
                                 const float* thres, float* out, void* ws, cudaStream_t s) {
   DpsrPlan* pl = (DpsrPlan*)plan;
   const int G = pl->G;
-  DpsrWS w = DpsrWS::from((char*)ws, G, pl->work);
+  DpsrWS w = DpsrWS::from((char*)ws, G, pl->work, B);
   const size_t G3 = (size_t)G * G * G, Gs = (size_t)G * G * (G / 2 + 1);
   const float cs = 1.0f / (float)G;  // torch: cubesize = 1.0 / size (fp32)
   const float inv_n3 = (float)(1.0 / (double)G3);
   const int nlut = 3 * (G / 2 + 1) * (G / 2 + 1);
-  cudaMemsetAsync(w.ras, 0, sizeof(float) * 3 * G3, s);
-  cudaMemsetAsync(w.red, 0, sizeof(double) * 4, s);
+  cudaMemsetAsync(w.red, 0, sizeof(double) * 4 * B, s);
   dpsr_filter_lut_kernel<<<(nlut + 255) / 256, 256, 0, s>>>(nlut, G, sig, w.lut);
-  if (N > 0) dpsr_scatter_kernel<<<(N + 255) / 256, 256, 0, s>>>(N, G, cs, V, Nrm, w.ras);
-  if (!use(pl->r2c3, w.fft_work, s) || cufftExecR2C(pl->r2c3, w.ras, (cufftComplex*)w.spec) != CUFFT_SUCCESS)
-    return cudaErrorUnknown;
-  dpsr_spectral_kernel<<<(unsigned)((Gs + 255) / 256), 256, 0, s>>>(G, w.lut, w.spec, w.phi_hat, 0);
-  if (!use(pl->c2r1, w.fft_work, s) || cufftExecC2R(pl->c2r1, (cufftComplex*)w.phi_hat, w.phi_raw) != CUFFT_SUCCESS)
-    return cudaErrorUnknown;
-  if (N > 0)
-    dpsr_gather_mean_kernel<<<(N + 255) / 256, 256, 0, s>>>(N, G, cs, inv_n3, V, w.phi_raw, w.red);
-  dpsr_finalize_kernel<<<(unsigned)((G3 + 255) / 256), 256, 0, s>>>(G3, N > 0 ? N : 1, inv_n3, w.phi_raw, w.red, mode,
-                                                                    thres, out, w.scal);
+  for (int k = 0; k < B; ++k) {
+    const float *Vk = V + (size_t)k * N * 3, *Nk = Nrm + (size_t)k * N * 3;
+    float* phi_raw = w.phi_raw + (size_t)k * G3;
+    double* red = w.red + 4 * k;
+    cudaMemsetAsync(w.ras, 0, sizeof(float) * 3 * G3, s);
+    if (N > 0) dpsr_scatter_kernel<<<(N + 255) / 256, 256, 0, s>>>(N, G, cs, Vk, Nk, w.ras);
+    if (!use(pl->r2c3, w.fft_work, s) || cufftExecR2C(pl->r2c3, w.ras, (cufftComplex*)w.spec) != CUFFT_SUCCESS)
+      return cudaErrorUnknown;
+    dpsr_spectral_kernel<<<(unsigned)((Gs + 255) / 256), 256, 0, s>>>(G, w.lut, w.spec, w.phi_hat, 0);
+    if (!use(pl->c2r1, w.fft_work, s) || cufftExecC2R(pl->c2r1, (cufftComplex*)w.phi_hat, phi_raw) != CUFFT_SUCCESS)
+      return cudaErrorUnknown;
+    if (N > 0)
+      dpsr_gather_mean_kernel<<<(N + 255) / 256, 256, 0, s>>>(N, G, cs, inv_n3, Vk, phi_raw, red);
+    dpsr_finalize_kernel<<<(unsigned)((G3 + 255) / 256), 256, 0, s>>>(G3, N > 0 ? N : 1, inv_n3, phi_raw, red, mode,
+                                                                      thres, out + (size_t)k * G3, w.scal + 8 * k);
+  }
   return cudaGetLastError();
 }
 
-cudaError_t launch_dpsr_backward(void* plan, int N, const float* V, const float* Nrm, int mode, const float* g,
+// g[B,G,G,G] -> dV[B,N,3], dN[B,N,3], dthres[B] (each item's own dL/dthres; may be NULL)
+cudaError_t launch_dpsr_backward(void* plan, int B, int N, const float* V, const float* Nrm, int mode, const float* g,
                                  float* dV, float* dN, float* dthres, void* ws, cudaStream_t s) {
   DpsrPlan* pl = (DpsrPlan*)plan;
   const int G = pl->G;
-  DpsrWS w = DpsrWS::from((char*)ws, G, pl->work);
+  DpsrWS w = DpsrWS::from((char*)ws, G, pl->work, B);
   const size_t G3 = (size_t)G * G * G, Gs = (size_t)G * G * (G / 2 + 1);
   const float cs = 1.0f / (float)G;
   const float inv_n3 = (float)(1.0 / (double)G3);
-  cudaMemsetAsync(w.red, 0, sizeof(double) * 4, s);
-  dpsr_bwd_reduce_kernel<<<592, 256, 0, s>>>(G3, inv_n3, g, w.phi_raw, w.scal, w.red);
-  dpsr_bwd_dphi_kernel<<<(unsigned)((G3 + 255) / 256), 256, 0, s>>>(G3, N > 0 ? N : 1, g, w.scal, w.red, mode, w.dphi,
-                                                                    w.scal + 2, dthres);
-  if (N > 0)
-    dpsr_bwd_interp_kernel<<<(N + 255) / 256, 256, 0, s>>>(N, G, cs, inv_n3, V, w.phi_raw, w.scal + 2, w.dphi, dV);
-  // adjoint spectral solve: rfftn(dphi) -> conj(H_c) -> irfftn per channel (into the ras buffer)
-  if (!use(pl->r2c1, w.fft_work, s) || cufftExecR2C(pl->r2c1, w.dphi, (cufftComplex*)w.phi_hat) != CUFFT_SUCCESS)
-    return cudaErrorUnknown;
-  dpsr_spectral_kernel<<<(unsigned)((Gs + 255) / 256), 256, 0, s>>>(G, w.lut, w.phi_hat, w.spec, 1);
-  if (!use(pl->c2r3, w.fft_work, s) || cufftExecC2R(pl->c2r3, (cufftComplex*)w.spec, w.ras) != CUFFT_SUCCESS)
-    return cudaErrorUnknown;
-  if (N > 0)
-    dpsr_bwd_points_kernel<<<(N + 255) / 256, 256, 0, s>>>(N, G, cs, inv_n3, V, Nrm, w.ras, dV, dN);
+  cudaMemsetAsync(w.red, 0, sizeof(double) * 4 * B, s);
+  for (int k = 0; k < B; ++k) {
+    const float *Vk = V + (size_t)k * N * 3, *Nk = Nrm + (size_t)k * N * 3, *gk = g + (size_t)k * G3;
+    float *dVk = dV + (size_t)k * N * 3, *dNk = dN + (size_t)k * N * 3;
+    const float* phi_raw = w.phi_raw + (size_t)k * G3;
+    double* red = w.red + 4 * k;
+    float* scal = w.scal + 8 * k;
+    dpsr_bwd_reduce_kernel<<<592, 256, 0, s>>>(G3, inv_n3, gk, phi_raw, scal, red);
+    dpsr_bwd_dphi_kernel<<<(unsigned)((G3 + 255) / 256), 256, 0, s>>>(G3, N > 0 ? N : 1, gk, scal, red, mode, w.dphi,
+                                                                      scal + 2, dthres ? dthres + k : nullptr);
+    if (N > 0)
+      dpsr_bwd_interp_kernel<<<(N + 255) / 256, 256, 0, s>>>(N, G, cs, inv_n3, Vk, phi_raw, scal + 2, w.dphi, dVk);
+    // adjoint spectral solve: rfftn(dphi) -> conj(H_c) -> irfftn per channel (into the ras buffer)
+    if (!use(pl->r2c1, w.fft_work, s) || cufftExecR2C(pl->r2c1, w.dphi, (cufftComplex*)w.phi_hat) != CUFFT_SUCCESS)
+      return cudaErrorUnknown;
+    dpsr_spectral_kernel<<<(unsigned)((Gs + 255) / 256), 256, 0, s>>>(G, w.lut, w.phi_hat, w.spec, 1);
+    if (!use(pl->c2r3, w.fft_work, s) || cufftExecC2R(pl->c2r3, (cufftComplex*)w.spec, w.ras) != CUFFT_SUCCESS)
+      return cudaErrorUnknown;
+    if (N > 0)
+      dpsr_bwd_points_kernel<<<(N + 255) / 256, 256, 0, s>>>(N, G, cs, inv_n3, Vk, Nk, w.ras, dVk, dNk);
+  }
   return cudaGetLastError();
 }
 

@@ -120,13 +120,16 @@ __device__ __forceinline__ void mc_classify(const McGeom& g, const McBrick& B, i
   }
 }
 
-__global__ void __launch_bounds__(32 * MC_WARPS) mc_count_kernel(McGeom g, const float* __restrict__ phi, float iso,
+// a batch of grids phi[items, G, G, G] is swept as items * nbricks bricks; brick b belongs to item b / nbricks
+__global__ void __launch_bounds__(32 * MC_WARPS) mc_count_kernel(McGeom g, size_t nall, const float* __restrict__ phi,
+                                                                 float iso,
                                                                  unsigned long long* __restrict__ blk_counts) {
   const unsigned lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const size_t brick = (size_t)blockIdx.x * MC_WARPS + wid;
-  if (brick >= g.nbricks) return;
+  if (brick >= nall) return;
+  const size_t item = brick / g.nbricks;
   McBrick B;
-  mc_load_brick(g, brick, lane, phi, B);
+  mc_load_brick(g, brick - item * g.nbricks, lane, phi + item * g.G * g.G * g.G, B);
   // the common case (>95 % of a 288^3 grid): every value the brick touches lies on one side of the level set --
   // nothing to classify.  Lanes look at their own valid values (lane 31 also at its k + 1 column).
   {
@@ -165,32 +168,47 @@ __global__ void __launch_bounds__(32 * MC_WARPS) mc_count_kernel(McGeom g, const
   if (lane == 0) blk_counts[brick] = (unsigned long long)(c & 0xffffu) | ((unsigned long long)(c >> 16) << 32);
 }
 
-// {V, F} -> the workspace copy (resolve pass), the caller's device copy and its host-mapped mirror
-__global__ void mc_totals_kernel(size_t nb, const unsigned long long* __restrict__ counts,
-                                 const unsigned long long* __restrict__ offsets, int32_t* __restrict__ ws_totals,
+// {V_k, F_k} of every item -> the workspace's item offsets (emit and resolve), the caller's device pairs and their
+// host-mapped mirror.  The difference of the packed prefix at an item's two ends is exactly V_k + 2^32 F_k
+// (V_k < 2^32), whatever the earlier items carried from the vertex half into the face half of the packed scan.
+__global__ void mc_totals_kernel(int B, size_t nb, const unsigned long long* __restrict__ counts,
+                                 const unsigned long long* __restrict__ offsets, long long* __restrict__ item_off,
                                  int32_t* __restrict__ totals, volatile int32_t* __restrict__ totals_host) {
-  const unsigned long long t = offsets[nb - 1] + counts[nb - 1];
-  const int32_t V = (int32_t)(t & 0xffffffffull), F = (int32_t)(t >> 32);
-  ws_totals[0] = V;
-  ws_totals[1] = F;
-  totals[0] = V;
-  totals[1] = F;
-  if (totals_host) {
-    totals_host[0] = V;
-    totals_host[1] = F;
-    __threadfence_system();
+  long long vo = 0, fo = 0;
+  for (int k = 0; k < B; ++k) {
+    const unsigned long long lo = offsets[k * nb];
+    const unsigned long long hi = k + 1 < B ? offsets[(k + 1) * nb] : offsets[B * nb - 1] + counts[B * nb - 1];
+    const unsigned long long d = hi - lo;
+    const int32_t V = (int32_t)(d & 0xffffffffull), F = (int32_t)(d >> 32);
+    item_off[k] = vo;
+    item_off[B + 1 + k] = fo;
+    vo += V;
+    fo += F;
+    totals[2 * k] = V;
+    totals[2 * k + 1] = F;
+    if (totals_host) {
+      totals_host[2 * k] = V;
+      totals_host[2 * k + 1] = F;
+    }
   }
+  item_off[B] = vo;
+  item_off[2 * B + 1] = fo;
+  if (totals_host) __threadfence_system();
 }
 
+// item k's vertices and faces follow those of items 0..k-1 (item_off); vid, vsrc and the face references are local
+// to the item, so item k's slice is what the item alone gives
 __global__ void __launch_bounds__(32 * MC_WARPS) mc_emit_kernel(
-    McGeom g, const float* __restrict__ phi, float iso, const unsigned long long* __restrict__ blk_counts,
-    const unsigned long long* __restrict__ blk_offsets, uint32_t* __restrict__ vid, float* __restrict__ verts,
-    int32_t* __restrict__ vsrc, long long V_cap, int32_t* __restrict__ faces, long long F_cap) {
+    McGeom g, int items, const float* __restrict__ phi, float iso, const unsigned long long* __restrict__ blk_counts,
+    const unsigned long long* __restrict__ blk_offsets, const long long* __restrict__ item_off,
+    uint32_t* __restrict__ vid, float* __restrict__ verts, int32_t* __restrict__ vsrc, long long V_cap,
+    int32_t* __restrict__ faces, long long F_cap) {
   const unsigned lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const size_t brick = (size_t)blockIdx.x * MC_WARPS + wid;
-  if (brick >= g.nbricks || blk_counts[brick] == 0) return;  // nothing owned here (the vast majority of bricks)
+  if (brick >= (size_t)items * g.nbricks || blk_counts[brick] == 0) return;  // nothing owned here (most bricks)
+  const size_t item = brick / g.nbricks, G3 = (size_t)g.G * g.G * g.G;
   McBrick B;
-  mc_load_brick(g, brick, lane, phi, B);
+  mc_load_brick(g, brick - item * g.nbricks, lane, phi + item * G3, B);
   unsigned masks = 0, css[MC_BJ];  // 3 bits of mask per node, packed
   unsigned mine = 0;
 #pragma unroll
@@ -208,9 +226,10 @@ __global__ void __launch_bounds__(32 * MC_WARPS) mc_emit_kernel(
   }
   if (mine == 0) return;
   const unsigned excl = inc - mine;
-  const unsigned long long base = blk_offsets[brick];
-  unsigned long long v = (base & 0xffffffffull) + (excl & 0xffffu);
-  unsigned long long f = (base >> 32) + (excl >> 16);
+  const unsigned long long base = blk_offsets[brick] - blk_offsets[item * g.nbricks];
+  unsigned long long vl = (base & 0xffffffffull) + (excl & 0xffffu);  // the item's own vertex index
+  const long long v0 = item_off[item];                               // + vl: the batch's vertex index
+  long long f = item_off[items + 1 + item] + (long long)(base >> 32) + (excl >> 16);
   const int G = g.G;
   const float gm1 = (float)(G - 1);
 #pragma unroll
@@ -220,14 +239,15 @@ __global__ void __launch_bounds__(32 * MC_WARPS) mc_emit_kernel(
     const int j = B.j0 + r;
     const size_t id = ((size_t)B.i * G + j) * G + B.k;
     if (mask) {
-      vid[id] = (uint32_t)v | (mask << 29);
+      vid[item * G3 + id] = (uint32_t)vl | (mask << 29);
       const float p0 = B.a[0][r];
       const float p1[3] = {B.a[1][r], B.a[0][r + 1], B.z[0][r]};
       const float basep[3] = {(float)B.i, (float)j, (float)B.k};
 #pragma unroll
       for (int a = 0; a < 3; ++a) {
         if (mask & (1u << a)) {
-          if ((long long)v < V_cap) {
+          const long long v = v0 + (long long)vl;
+          if (v < V_cap) {
             const float t = (iso - p0) / (p1[a] - p0);
             float pos[3] = {basep[0], basep[1], basep[2]};
             pos[a] += t;
@@ -236,13 +256,13 @@ __global__ void __launch_bounds__(32 * MC_WARPS) mc_emit_kernel(
             verts[3 * v + 2] = pos[2] / gm1;
             vsrc[v] = (int32_t)(id * 3 + a);  // < 3 G^3 < 2^31 for G <= 800
           }
-          ++v;
+          ++vl;
         }
       }
     }
     const int nt = (int)mc_ntri(cs);
     for (int t = 0; t < nt; ++t, ++f) {
-      if ((long long)f >= F_cap) break;
+      if (f >= F_cap) break;
 #pragma unroll
       for (int q = 0; q < 3; ++q) {
         const int e = __ldg(&g_tri[cs][3 * t + q]);
@@ -254,24 +274,41 @@ __global__ void __launch_bounds__(32 * MC_WARPS) mc_emit_kernel(
   }
 }
 
-__global__ void __launch_bounds__(256) mc_resolve_kernel(const int32_t* __restrict__ totals, long long F_cap,
-                                                         const uint32_t* __restrict__ vid,
+// foff = item_off + items + 1: the batch's first face of every item, and the total
+__global__ void __launch_bounds__(256) mc_resolve_kernel(int items, size_t G3, const long long* __restrict__ foff,
+                                                         long long F_cap, const uint32_t* __restrict__ vid,
                                                          int32_t* __restrict__ faces) {
-  const long long n = 3 * min((long long)totals[1], F_cap);
+  const long long n = 3 * min(foff[items], F_cap);
   const long long x = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (x >= n) return;
+  int lo = 0, hi = items - 1;  // the item of face x / 3: the last k with foff[k] <= x / 3
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (foff[mid] <= x / 3) lo = mid;
+    else hi = mid - 1;
+  }
   const uint32_t e = (uint32_t)faces[x];
-  const uint32_t w = vid[e / 3];
+  const uint32_t w = vid[(size_t)lo * G3 + e / 3];
   faces[x] = (int32_t)((w & 0x1fffffffu) + __popc((w >> 29) & ((1u << (e % 3)) - 1u)));
 }
 
 // dL/dphi += dL/dverts . d verts/d phi   (only the coordinate along the edge moves); one thread per vertex
-__global__ void __launch_bounds__(256) mc_backward_kernel(int G, int V, const float* __restrict__ phi, float iso,
+// item k's vertices are [it.voff[k], it.voff[k + 1]) of the batch, its grids phi / dphi + k G^3
+__global__ void __launch_bounds__(256) mc_backward_kernel(int G, McItems it, const float* __restrict__ phi, float iso,
                                                           const int32_t* __restrict__ vsrc,
                                                           const float* __restrict__ dverts,
                                                           float* __restrict__ dphi) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= V) return;
+  if (v >= it.voff[it.B]) return;
+  int lo = 0, hi = it.B - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (it.voff[mid] <= v) lo = mid;
+    else hi = mid - 1;
+  }
+  const size_t G3 = (size_t)G * G * G;
+  phi += lo * G3;
+  dphi += lo * G3;
   const uint32_t e = (uint32_t)vsrc[v];
   const size_t id = e / 3;
   const int a = (int)(e % 3);
@@ -309,52 +346,56 @@ size_t mc_cub_bytes(size_t n) {
   return bytes;
 }
 
-McWS McWS::from(char* base, int G, size_t* bytes) {
+McWS McWS::from(char* base, int G, int B, size_t* bytes) {
   char* p = base;
   McWS w;
-  const size_t n = (size_t)G * G * G, nb = mc_num_blocks(G);
+  const size_t n = (size_t)G * G * G, nb = (size_t)B * mc_num_blocks(G);
   w.blk_counts = carve<unsigned long long>(p, nb);
   w.blk_offsets = carve<unsigned long long>(p, nb);
-  w.totals = carve<int32_t>(p, 4);
+  w.item_off = carve<long long>(p, 2 * (size_t)B + 2);
   w.cub_bytes = mc_cub_bytes(nb);
   w.cub_temp = carve<char>(p, w.cub_bytes);
-  w.vid = carve<uint32_t>(p, n);    // sparse: only entries of vertex-owning nodes are ever written or read
+  w.vid = carve<uint32_t>(p, (size_t)B * n);    // sparse: only entries of vertex-owning nodes are ever written or read
   if (bytes) *bytes = size_t(p - base) + 128;
   return w;
 }
 
-cudaError_t launch_mc_count(int G, const float* phi, float iso, void* ws, int32_t* totals, int32_t* totals_host,
-                            cudaEvent_t ev, cudaStream_t s) {
+cudaError_t launch_mc_count(int B, int G, const float* phi, float iso, void* ws, int32_t* totals,
+                            int32_t* totals_host, cudaEvent_t ev, cudaStream_t s) {
   cudaError_t e = upload_tables();
   if (e != cudaSuccess) return e;
-  McWS w = McWS::from((char*)ws, G);
+  McWS w = McWS::from((char*)ws, G, B);
   const McGeom g = mc_geom(G);
-  const size_t nb = mc_num_blocks(G);
-  mc_count_kernel<<<(unsigned)((nb + MC_WARPS - 1) / MC_WARPS), 32 * MC_WARPS, 0, s>>>(g, phi, iso, w.blk_counts);
+  const size_t nb = mc_num_blocks(G), nall = (size_t)B * nb;
+  mc_count_kernel<<<(unsigned)((nall + MC_WARPS - 1) / MC_WARPS), 32 * MC_WARPS, 0, s>>>(g, nall, phi, iso,
+                                                                                          w.blk_counts);
   size_t tb = w.cub_bytes;
-  cub::DeviceScan::ExclusiveSum(w.cub_temp, tb, w.blk_counts, w.blk_offsets, (int)nb, s);
-  mc_totals_kernel<<<1, 1, 0, s>>>(nb, w.blk_counts, w.blk_offsets, w.totals, totals, (volatile int32_t*)totals_host);
+  cub::DeviceScan::ExclusiveSum(w.cub_temp, tb, w.blk_counts, w.blk_offsets, (int)nall, s);
+  mc_totals_kernel<<<1, 1, 0, s>>>(B, nb, w.blk_counts, w.blk_offsets, w.item_off, totals,
+                                   (volatile int32_t*)totals_host);
   if (ev) cudaEventRecord(ev, s);
   return cudaGetLastError();
 }
 
-cudaError_t launch_mc_emit(int G, const float* phi, float iso, void* ws, float* verts, int32_t* vsrc,
+cudaError_t launch_mc_emit(int B, int G, const float* phi, float iso, void* ws, float* verts, int32_t* vsrc,
                            long long V_cap, int32_t* faces, long long F_cap, cudaStream_t s) {
-  McWS w = McWS::from((char*)ws, G);
+  McWS w = McWS::from((char*)ws, G, B);
   const McGeom g = mc_geom(G);
-  const size_t nb = mc_num_blocks(G);
-  mc_emit_kernel<<<(unsigned)((nb + MC_WARPS - 1) / MC_WARPS), 32 * MC_WARPS, 0, s>>>(
-      g, phi, iso, w.blk_counts, w.blk_offsets, w.vid, verts, vsrc, V_cap, faces, F_cap);
+  const size_t nall = (size_t)B * mc_num_blocks(G);
+  mc_emit_kernel<<<(unsigned)((nall + MC_WARPS - 1) / MC_WARPS), 32 * MC_WARPS, 0, s>>>(
+      g, B, phi, iso, w.blk_counts, w.blk_offsets, w.item_off, w.vid, verts, vsrc, V_cap, faces, F_cap);
   if (F_cap > 0)
-    mc_resolve_kernel<<<(unsigned)((3 * F_cap + 255) / 256), 256, 0, s>>>(w.totals, F_cap, w.vid, faces);
+    mc_resolve_kernel<<<(unsigned)((3 * F_cap + 255) / 256), 256, 0, s>>>(B, (size_t)G * G * G, w.item_off + B + 1,
+                                                                          F_cap, w.vid, faces);
   return cudaGetLastError();
 }
 
-cudaError_t launch_mc_backward(int G, int V, const float* phi, float iso, const int32_t* vsrc, const float* dverts,
-                               float* dphi, cudaStream_t s) {
-  const size_t n = (size_t)G * G * G;
+cudaError_t launch_mc_backward(int G, const McItems& it, const float* phi, float iso, const int32_t* vsrc,
+                               const float* dverts, float* dphi, cudaStream_t s) {
+  const size_t n = (size_t)it.B * G * G * G;
+  const int V = it.voff[it.B];
   cudaMemsetAsync(dphi, 0, sizeof(float) * n, s);
-  if (V > 0) mc_backward_kernel<<<(V + 255) / 256, 256, 0, s>>>(G, V, phi, iso, vsrc, dverts, dphi);
+  if (V > 0) mc_backward_kernel<<<(V + 255) / 256, 256, 0, s>>>(G, it, phi, iso, vsrc, dverts, dphi);
   return cudaGetLastError();
 }
 

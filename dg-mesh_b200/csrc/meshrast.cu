@@ -42,6 +42,16 @@ __device__ __forceinline__ float edge_fn(float ax, float ay, float bx, float by,
   return (bx - ax) * (py - ay) - (by - ay) * (px - ax);
 }
 
+// rast.w holds triangle id + 1 as nvdiffrast encodes it: as a float up to 2^24, where every integer is exact, and
+// above that as the float whose bit pattern is 0x4a800000 + (id + 1) (larger than 2^24 and increasing with the id),
+// so an id past 2^24 never reads as a neighbouring triangle's.  Ids up to MR_MAX_TRIANGLES keep the pattern finite.
+__device__ __forceinline__ float mr_id_to_float(int x) {
+  return x <= 0x01000000 ? (float)x : __int_as_float(0x4a800000 + x);
+}
+__device__ __forceinline__ int mr_float_to_id(float x) {
+  return x <= 16777216.0f ? (int)x : __float_as_int(x) - 0x4a800000;
+}
+
 // positive floats and zero order like their bit patterns; map [-1, 1] to [0, 2] first
 __device__ __forceinline__ uint32_t depth_key(float zw) { return __float_as_uint(zw + 1.0f); }
 
@@ -50,11 +60,21 @@ __global__ void __launch_bounds__(256) mr_clear_kernel(size_t n, unsigned long l
   if (i < n) zbuf[i] = ~0ull;
 }
 
-__global__ void __launch_bounds__(128) mr_raster_kernel(int F, int W, int H, const float* __restrict__ pos,
+// one thread per (image, triangle of its range): thread t < R.off[R.B] draws triangle R.start[b] + t - R.off[b] into
+// image b's z-buffer
+__global__ void __launch_bounds__(128) mr_raster_kernel(MrRanges R, int W, int H, const float* __restrict__ pos,
                                                         const int* __restrict__ tri,
                                                         unsigned long long* __restrict__ zbuf) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= F) return;
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= R.off[R.B]) return;
+  int img = 0, hi = R.B - 1;  // the last image whose first thread is <= t (empty ranges own no thread)
+  while (img < hi) {
+    const int mid = (img + hi + 1) >> 1;
+    if (R.off[mid] <= t) img = mid;
+    else hi = mid - 1;
+  }
+  const int f = R.start[img] + (t - R.off[img]);
+  zbuf += (size_t)img * W * H;
   const int i0 = tri[3 * f], i1 = tri[3 * f + 1], i2 = tri[3 * f + 2];
   const MrVert a = mr_project(pos, i0, W, H), b = mr_project(pos, i1, W, H), c = mr_project(pos, i2, W, H);
   if (a.iw <= 0.f || b.iw <= 0.f || c.iw <= 0.f) return;  // no clipping: the mesh is in front of the camera
@@ -92,13 +112,14 @@ __device__ __forceinline__ void mr_bary(const MrVert& a, const MrVert& b, const 
   zw = b0 * a.zw + b1 * b.zw + b2 * c.zw;
 }
 
+// image blockIdx.z; triangle ids are global
 __global__ void __launch_bounds__(256) mr_resolve_kernel(int W, int H, const float* __restrict__ pos,
                                                          const int* __restrict__ tri,
                                                          const unsigned long long* __restrict__ zbuf,
                                                          float4* __restrict__ rast) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= W || y >= H) return;
-  const size_t p = (size_t)y * W + x;
+  const size_t p = ((size_t)blockIdx.z * H + y) * W + x;
   const unsigned long long k = zbuf[p];
   if (k == ~0ull) {
     rast[p] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -109,16 +130,18 @@ __global__ void __launch_bounds__(256) mr_resolve_kernel(int W, int H, const flo
                c = mr_project(pos, tri[3 * f + 2], W, H);
   float u, v, zw;
   mr_bary(a, b, c, x + 0.5f, y + 0.5f, u, v, zw);
-  rast[p] = make_float4(u, v, zw, (float)(f + 1));
+  rast[p] = make_float4(u, v, zw, mr_id_to_float(f + 1));
 }
 
-cudaError_t launch_mr_rasterize(int V, int F, int W, int H, const float* pos, const int* tri, void* zbuf, float* rast,
-                                cudaStream_t s) {
-  const size_t n = (size_t)W * H;
+cudaError_t launch_mr_rasterize(const MrRanges& R, int W, int H, const float* pos, const int* tri, void* zbuf,
+                                float* rast, cudaStream_t s) {
+  const size_t n = (size_t)R.B * W * H;
+  const int T = R.off[R.B];
   mr_clear_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(n, (unsigned long long*)zbuf);
-  if (F > 0) mr_raster_kernel<<<(F + 127) / 128, 128, 0, s>>>(F, W, H, pos, tri, (unsigned long long*)zbuf);
-  mr_resolve_kernel<<<dim3((W + 31) / 32, (H + 7) / 8), 256, 0, s>>>(W, H, pos, tri, (const unsigned long long*)zbuf,
-                                                                     (float4*)rast);
+  if (T > 0) mr_raster_kernel<<<(T + 127) / 128, 128, 0, s>>>(R, W, H, pos, tri, (unsigned long long*)zbuf);
+  mr_resolve_kernel<<<dim3((W + 31) / 32, (H + 7) / 8, R.B), 256, 0, s>>>(W, H, pos, tri,
+                                                                          (const unsigned long long*)zbuf,
+                                                                          (float4*)rast);
   return cudaGetLastError();
 }
 
@@ -202,13 +225,14 @@ __device__ __forceinline__ void mr_bary_backward(const float4 ca, const float4 c
 }
 
 // ---------------------------------------------------------------- interpolate
-__global__ void __launch_bounds__(256) mr_interp_fwd_kernel(int W, int H, int C, const float* __restrict__ attr,
+// interpolate and its backward are per pixel: n = B W H pixels of B images
+__global__ void __launch_bounds__(256) mr_interp_fwd_kernel(size_t n, int C, const float* __restrict__ attr,
                                                             const float4* __restrict__ rast,
                                                             const int* __restrict__ tri, float* __restrict__ out) {
   const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= (size_t)W * H) return;
+  if (p >= n) return;
   const float4 r = rast[p];
-  const int f = (int)r.w - 1;
+  const int f = mr_float_to_id(r.w) - 1;
   if (f < 0) {
     for (int ch = 0; ch < C; ++ch) out[p * C + ch] = 0.f;
     return;
@@ -220,14 +244,14 @@ __global__ void __launch_bounds__(256) mr_interp_fwd_kernel(int W, int H, int C,
 }
 
 // dL/dout -> dL/dattr (atomics) and dL/drast = (dL/du, dL/dv, 0, 0), fully written
-__global__ void __launch_bounds__(256) mr_interp_bwd_kernel(int W, int H, int C, const float* __restrict__ attr,
+__global__ void __launch_bounds__(256) mr_interp_bwd_kernel(size_t n, int C, const float* __restrict__ attr,
                                                             const float4* __restrict__ rast,
                                                             const int* __restrict__ tri, const float* __restrict__ gout,
                                                             float* __restrict__ gattr, float4* __restrict__ grast) {
   const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= (size_t)W * H) return;
+  if (p >= n) return;
   const float4 r = rast[p];
-  const int f = (int)r.w - 1;
+  const int f = mr_float_to_id(r.w) - 1;
   float gu = 0.f, gv = 0.f;
   if (f >= 0) {
     const int idx[3] = {tri[3 * f], tri[3 * f + 1], tri[3 * f + 2]};
@@ -249,20 +273,20 @@ __global__ void __launch_bounds__(256) mr_interp_bwd_kernel(int W, int H, int C,
   if (grast) grast[p] = make_float4(gu, gv, 0.f, 0.f);
 }
 
-// rasterize backward: dL/d(u, v) per pixel -> dL/dpos (clip space, atomics; z gets no gradient)
-__global__ void __launch_bounds__(256) mr_raster_bwd_kernel(int W, int H, const float4* __restrict__ rast,
+// rasterize backward: dL/d(u, v) per pixel of B images -> dL/dpos (clip space, atomics; z gets no gradient)
+__global__ void __launch_bounds__(256) mr_raster_bwd_kernel(int B, int W, int H, const float4* __restrict__ rast,
                                                             const int* __restrict__ tri, const float* __restrict__ pos,
                                                             const float4* __restrict__ grast, float* __restrict__ gpos) {
   const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= (size_t)W * H) return;
-  const int f = (int)rast[p].w - 1;
+  if (p >= (size_t)B * W * H) return;
+  const int f = mr_float_to_id(rast[p].w) - 1;
   if (f < 0) return;
   const float4 gr = grast[p];
   if (gr.x == 0.f && gr.y == 0.f) return;
   const int idx[3] = {tri[3 * f], tri[3 * f + 1], tri[3 * f + 2]};
   const float4* P4 = reinterpret_cast<const float4*>(pos);
   float g[3][4];
-  const int x = (int)(p % W), y = (int)(p / W);
+  const int x = (int)(p % W), y = (int)((p / W) % H);
   mr_bary_backward(P4[idx[0]], P4[idx[1]], P4[idx[2]], W, H, x + 0.5f, y + 0.5f, gr.x, gr.y, g);
 #pragma unroll
   for (int i = 0; i < 3; ++i) {
@@ -272,25 +296,25 @@ __global__ void __launch_bounds__(256) mr_raster_bwd_kernel(int W, int H, const 
   }
 }
 
-cudaError_t launch_mr_interpolate(int W, int H, int C, const float* attr, const float* rast, const int* tri,
+cudaError_t launch_mr_interpolate(int B, int W, int H, int C, const float* attr, const float* rast, const int* tri,
                                   float* out, cudaStream_t s) {
-  const size_t n = (size_t)W * H;
-  mr_interp_fwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(W, H, C, attr, (const float4*)rast, tri, out);
+  const size_t n = (size_t)B * W * H;
+  mr_interp_fwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(n, C, attr, (const float4*)rast, tri, out);
   return cudaGetLastError();
 }
 
-cudaError_t launch_mr_interpolate_bwd(int W, int H, int C, const float* attr, const float* rast, const int* tri,
+cudaError_t launch_mr_interpolate_bwd(int B, int W, int H, int C, const float* attr, const float* rast, const int* tri,
                                       const float* gout, float* gattr, float* grast, cudaStream_t s) {
-  const size_t n = (size_t)W * H;
-  mr_interp_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(W, H, C, attr, (const float4*)rast, tri, gout,
-                                                                   gattr, (float4*)grast);
+  const size_t n = (size_t)B * W * H;
+  mr_interp_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(n, C, attr, (const float4*)rast, tri, gout, gattr,
+                                                                   (float4*)grast);
   return cudaGetLastError();
 }
 
-cudaError_t launch_mr_rasterize_bwd(int W, int H, const float* rast, const int* tri, const float* pos,
+cudaError_t launch_mr_rasterize_bwd(int B, int W, int H, const float* rast, const int* tri, const float* pos,
                                     const float* grast, float* gpos, cudaStream_t s) {
-  const size_t n = (size_t)W * H;
-  mr_raster_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(W, H, (const float4*)rast, tri, pos,
+  const size_t n = (size_t)B * W * H;
+  mr_raster_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(B, W, H, (const float4*)rast, tri, pos,
                                                                    (const float4*)grast, gpos);
   return cudaGetLastError();
 }
@@ -318,7 +342,7 @@ __device__ __forceinline__ AaPair aa_pair(int x, int y, int dir, int W, int H, c
   if (x1 >= W || y1 >= H) return r;
   const int p0 = y * W + x, p1 = y1 * W + x1;
   const float4 r0 = rast[p0], r1 = rast[p1];
-  const int f0 = (int)r0.w - 1, f1 = (int)r1.w - 1;
+  const int f0 = mr_float_to_id(r0.w) - 1, f1 = mr_float_to_id(r1.w) - 1;
   if (f0 == f1) return r;
   // the nearer surface owns the boundary
   const bool first_in = (f1 < 0) || (f0 >= 0 && r0.z <= r1.z);
@@ -386,14 +410,18 @@ __device__ __forceinline__ AaPair aa_pair(int x, int y, int dir, int W, int H, c
   return r;
 }
 
-__global__ void __launch_bounds__(256) mr_aa_fwd_kernel(int W, int H, int C, const float* __restrict__ color,
+// B images: thread i pairs within image (i / 2) / (W H) only, so no pair spans two images
+__global__ void __launch_bounds__(256) mr_aa_fwd_kernel(int B, int W, int H, int C, const float* __restrict__ color,
                                                         const float4* __restrict__ rast,
                                                         const float* __restrict__ pos, const int* __restrict__ tri,
                                                         const int* __restrict__ opp, float* __restrict__ out) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (size_t)W * H * 2) return;
+  if (i >= (size_t)B * W * H * 2) return;
   const int dir = (int)(i & 1);
-  const size_t p = i >> 1;
+  const size_t n = (size_t)W * H, b = (i >> 1) / n, p = (i >> 1) - b * n;
+  color += b * n * C;
+  rast += b * n;
+  out += b * n * C;
   const AaPair a = aa_pair((int)(p % W), (int)(p / W), dir, W, H, rast, pos, tri, opp);
   if (!a.valid || a.wgt == 0.f) return;
   const int src = (a.dst == a.p_in) ? a.p_out : a.p_in;
@@ -403,15 +431,19 @@ __global__ void __launch_bounds__(256) mr_aa_fwd_kernel(int W, int H, int C, con
   }
 }
 
-__global__ void __launch_bounds__(256) mr_aa_bwd_kernel(int W, int H, int C, const float* __restrict__ color,
+__global__ void __launch_bounds__(256) mr_aa_bwd_kernel(int B, int W, int H, int C, const float* __restrict__ color,
                                                         const float4* __restrict__ rast,
                                                         const float* __restrict__ pos, const int* __restrict__ tri,
                                                         const int* __restrict__ opp, const float* __restrict__ gout,
                                                         float* __restrict__ gcolor, float* __restrict__ gpos) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (size_t)W * H * 2) return;
+  if (i >= (size_t)B * W * H * 2) return;
   const int dir = (int)(i & 1);
-  const size_t p = i >> 1;
+  const size_t n = (size_t)W * H, b = (i >> 1) / n, p = (i >> 1) - b * n;
+  color += b * n * C;
+  rast += b * n;
+  gout += b * n * C;
+  if (gcolor) gcolor += b * n * C;
   const AaPair a = aa_pair((int)(p % W), (int)(p / W), dir, W, H, rast, pos, tri, opp);
   if (!a.valid) return;
   const int src = (a.dst == a.p_in) ? a.p_out : a.p_in;
@@ -443,22 +475,22 @@ __global__ void __launch_bounds__(256) mr_aa_bwd_kernel(int W, int H, int C, con
   }
 }
 
-cudaError_t launch_mr_antialias(int W, int H, int C, const float* color, const float* rast, const float* pos,
+cudaError_t launch_mr_antialias(int B, int W, int H, int C, const float* color, const float* rast, const float* pos,
                                 const int* tri, const int* opp, float* out, cudaStream_t s) {
-  const size_t n = (size_t)W * H;
+  const size_t n = (size_t)B * W * H;
   cudaMemcpyAsync(out, color, sizeof(float) * n * C, cudaMemcpyDeviceToDevice, s);
-  mr_aa_fwd_kernel<<<(unsigned)((2 * n + 255) / 256), 256, 0, s>>>(W, H, C, color, (const float4*)rast, pos, tri, opp,
-                                                                   out);
+  mr_aa_fwd_kernel<<<(unsigned)((2 * n + 255) / 256), 256, 0, s>>>(B, W, H, C, color, (const float4*)rast, pos, tri,
+                                                                   opp, out);
   return cudaGetLastError();
 }
 
-cudaError_t launch_mr_antialias_bwd(int W, int H, int C, const float* color, const float* rast, const float* pos,
+cudaError_t launch_mr_antialias_bwd(int B, int W, int H, int C, const float* color, const float* rast, const float* pos,
                                     const int* tri, const int* opp, const float* gout, float* gcolor, float* gpos,
                                     cudaStream_t s) {
-  const size_t n = (size_t)W * H;
+  const size_t n = (size_t)B * W * H;
   if (gcolor) cudaMemcpyAsync(gcolor, gout, sizeof(float) * n * C, cudaMemcpyDeviceToDevice, s);
-  mr_aa_bwd_kernel<<<(unsigned)((2 * n + 255) / 256), 256, 0, s>>>(W, H, C, color, (const float4*)rast, pos, tri, opp,
-                                                                   gout, gcolor, gpos);
+  mr_aa_bwd_kernel<<<(unsigned)((2 * n + 255) / 256), 256, 0, s>>>(B, W, H, C, color, (const float4*)rast, pos, tri,
+                                                                   opp, gout, gcolor, gpos);
   return cudaGetLastError();
 }
 

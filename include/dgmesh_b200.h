@@ -807,7 +807,7 @@ int dgk_nearest(int Q, const float* queries, int R, const float* refs,
  * DPSR -- differentiable Poisson surface reconstruction on a G^3 periodic grid.
  * replaces DPSR.forward (dgmesh/nvdiffrast_utils/dpsr.py:28-70) with point_rasterize /
  * grid_interp / spec_gaussian_filter / fftfreqs (dgmesh/nvdiffrast_utils/dpsr_utils.py:25-197)
- * and the autograd graph PyTorch builds through them.  Batch size 1 (what DG-Mesh uses).
+ * and the autograd graph PyTorch builds through them.  One item here; the _batch calls below take B.
  *   V[N,3] in (0,1), Nrm[N,3]  ->  out[G,G,G]
  *   mode 0: out = phi exactly as DPSR.forward returns it (shifted, scaled by -0.5/|phi[0,0,0]|)
  *   mode 1: out = psr * sign - thres[0] as mesh_renderer forms it (dgmesh/utils/renderer.py:
@@ -824,6 +824,25 @@ int dgp_forward(void* plan, int N, double sig, const float* V, const float* Nrm,
 int dgp_backward(void* plan, int N, const float* V, const float* Nrm, int mode,
                  const float* dL_dout, float* dV, float* dN, float* dthres,
                  void* ws, size_t ws_bytes, void* stream);
+/* DPSR over a batch of B point sets (the reference's DPSR.forward(V[b,nv,3], N[b,nv,3])), 1 <= B <= 64; B out
+ * of range, a NULL pointer or a short workspace is refused on the host before any device work.
+ *   V[B,N,3], Nrm[B,N,3]  ->  out[B,G,G,G]; every item is normalised on its own (its own offset and its own
+ *   phi[k,0,0,0] scale, or in mode 1 its own sign from psr[k,0,0,0]); item k equals the single call on item k.
+ *   All items share thres[0] (mode 1).
+ * dgp_batch_workspace_size: bytes of a B-item workspace for the plan's G.  Only each item's field (4 G^3 bytes)
+ * and a few scalars outlive the forward; the spectra, the normals grid and the FFT work area are scratch that
+ * the items reuse one after another, so the size is the single-item size plus 4 G^3 (B - 1) bytes (at G = 288:
+ * 0.86 GB + 95.6 MB per further item).  B = 1 gives dgp_plan_create's ws_bytes.  dgp_forward_batch and
+ * dgp_backward_batch must be given the same workspace.
+ * dgp_backward_batch: dL_dout[B,G,G,G] -> dV[B,N,3], dN[B,N,3], dthres[B] (mode 1: each item's own dL/dthres,
+ * which the caller sums for the shared threshold; may be NULL).
+ * dgp_forward / dgp_backward are the B = 1 calls of the same launchers. */
+int dgp_batch_workspace_size(void* plan, int B, size_t* bytes);
+int dgp_forward_batch(void* plan, int B, int N, double sig, const float* V, const float* Nrm, int mode,
+                      const float* thres, float* out, void* ws, size_t ws_bytes, void* stream);
+int dgp_backward_batch(void* plan, int B, int N, const float* V, const float* Nrm, int mode,
+                       const float* dL_dout, float* dV, float* dN, float* dthres,
+                       void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------
  * Differentiable marching cubes.  Stands in for diso.DiffMC.__call__(grid, deform=None,
@@ -851,6 +870,26 @@ int dgmc_emit(int G, const float* phi, float iso, void* ws, size_t ws_bytes,
               float* verts, int32_t* vsrc, int64_t V_cap, int32_t* faces, int64_t F_cap, void* stream);
 int dgmc_backward(int G, int V, const float* phi, float iso, const int32_t* vsrc,
                   const float* dL_dverts, float* dL_dphi, void* stream);
+/* Marching cubes over a batch of B grids phi[B,G,G,G], 1 <= B <= 64 (B out of range, a NULL pointer or a short
+ * workspace is refused on the host before any device work).  The count pass sweeps all B grids in one launch,
+ * one scan covers the B grids' brick totals, and one kernel writes totals[B,2] = {V_k, F_k} of every item (and
+ * the same pairs to totals_host behind totals_event: dgm_notify_host has room for 256 pairs).  dgmc_emit_batch
+ * writes the items one after another -- item k's vertices start at V_0 + .. + V_(k-1), its faces at
+ * F_0 + .. + F_(k-1) -- with face indices LOCAL to the item and vsrc local to the item's grid, so item k's slice
+ * is exactly what dgmc_emit gives for grid k.  The capacities bound the batch's totals: the 29-bit vertex
+ * packing limits the WHOLE batch to V_0 + .. + V_(B-1) <= 2^29 vertices (V_cap <= 2^29), and F_cap < 2^31.
+ * dgmc_backward_batch: V_host[B] (host) = the items' vertex counts from totals; dL_dverts[V,3] of the concatenated
+ * vertices -> dL_dphi[B,G,G,G] (fully written), one launch.
+ * dgmc_workspace_size_batch at B = 1 equals dgmc_workspace_size, and every further item adds its own vertex-owner
+ * table (4 G^3 bytes) and brick totals: about 97 MB per item at G = 288.  The single-grid entry points are the
+ * B = 1 calls of the same launchers. */
+int dgmc_workspace_size_batch(int B, int G, size_t* bytes);
+int dgmc_count_batch(int B, int G, const float* phi, float iso, void* ws, size_t ws_bytes,
+                     int32_t* totals, int32_t* totals_host, void* totals_event, void* stream);
+int dgmc_emit_batch(int B, int G, const float* phi, float iso, void* ws, size_t ws_bytes,
+                    float* verts, int32_t* vsrc, int64_t V_cap, int32_t* faces, int64_t F_cap, void* stream);
+int dgmc_backward_batch(int B, int G, const int32_t* V_host, const float* phi, float iso, const int32_t* vsrc,
+                        const float* dL_dverts, float* dL_dphi, void* stream);
 
 /* ------------------------------------------------------------------------
  * Tensor-core GEMM building blocks of the MLPs (wgmma, bf16 operands, fp32 accumulation in
@@ -1019,6 +1058,29 @@ int dgmr_antialias(int W, int H, int C, const float* color, const float* rast, c
 int dgmr_antialias_bwd(int W, int H, int C, const float* color, const float* rast, const float* pos,
                        const int32_t* tri, const int32_t* opp, const float* gout, float* gcolor, float* gpos,
                        void* stream);
+/* Range mode (nvdiffrast's way of rendering several meshes into a batch of images): B images, 1 <= B <= 64.
+ *   ranges[B,2] int32 on the HOST = (first triangle, count) of image b within tri[F,3]; every range must lie in
+ *   [0, F] (else DGM_E_BADARG before any device work).  The ranges are passed to the kernel by value.
+ *   dgmr_rasterize_batch   zbuf: 8 * B * H * W bytes -> rast[B,H,W,4], triangle ids GLOBAL + 1; an empty range
+ *                          gives an all-zero image
+ *   rast.w (both modes) holds id + 1 as nvdiffrast encodes it: a float up to 2^24, above that the float whose bit
+ *   pattern is 0x4a800000 + (id + 1); F <= 2^29 (larger F is refused).
+ *   the other _batch calls take rast[B,H,W,4] and images [B,H,W,C] and the same pos[V,4] / attr[V,C] / tri for
+ *   every image; gradients of pos and attr accumulate over the images.  Antialiasing pairs pixels within an
+ *   image only.  The single-image entry points are the B = 1 calls of the same launchers. */
+int dgmr_rasterize_batch(int V, int F, int B, const int32_t* ranges, int W, int H, const float* pos,
+                         const int32_t* tri, void* zbuf, float* rast, void* stream);
+int dgmr_rasterize_bwd_batch(int B, int W, int H, const float* rast, const int32_t* tri, const float* pos,
+                             const float* grast, float* gpos, void* stream);
+int dgmr_interpolate_batch(int B, int W, int H, int C, const float* attr, const float* rast, const int32_t* tri,
+                           float* out, void* stream);
+int dgmr_interpolate_bwd_batch(int B, int W, int H, int C, const float* attr, const float* rast,
+                               const int32_t* tri, const float* gout, float* gattr, float* grast, void* stream);
+int dgmr_antialias_batch(int B, int W, int H, int C, const float* color, const float* rast, const float* pos,
+                         const int32_t* tri, const int32_t* opp, float* out, void* stream);
+int dgmr_antialias_bwd_batch(int B, int W, int H, int C, const float* color, const float* rast, const float* pos,
+                             const int32_t* tri, const int32_t* opp, const float* gout, float* gcolor,
+                             float* gpos, void* stream);
 
 /* ------------------------------------------------------------------------
  * Adaptive density control on the device (next-tier row SURVEY.md 8(f)-2): the whole of
