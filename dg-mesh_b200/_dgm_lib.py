@@ -92,6 +92,14 @@ SIGNATURES = {
     "dgmc_count": (c_int, [c_int, P, c_float, P, c_size_t, P, P, P, P]),
     "dgmc_emit": (c_int, [c_int, P, c_float, P, c_size_t, P, P, c_int64, P, c_int64, P]),
     "dgmc_backward": (c_int, [c_int, c_int, P, c_float, P, P, P, P]),
+    "dgdmc_workspace_size": (c_int, [c_int, ctypes.POINTER(c_size_t)]),
+    "dgdmc_workspace_size_batch": (c_int, [c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "dgdmc_count": (c_int, [c_int, P, c_float, P, c_size_t, P, P, P, P]),
+    "dgdmc_count_batch": (c_int, [c_int, c_int, P, c_float, P, c_size_t, P, P, P, P]),
+    "dgdmc_emit": (c_int, [c_int, P, c_float, P, c_size_t, P, P, c_int64, P, P, c_int64, P]),
+    "dgdmc_emit_batch": (c_int, [c_int, c_int, P, c_float, P, c_size_t, P, P, c_int64, P, P, c_int64, P]),
+    "dgdmc_backward": (c_int, [c_int, c_int, P, c_float, P, c_size_t, P, P, P, P]),
+    "dgdmc_backward_batch": (c_int, [c_int, c_int, P, P, c_float, P, c_size_t, P, P, P, P]),
     "dgmc_workspace_size_batch": (c_int, [c_int, c_int, ctypes.POINTER(c_size_t)]),
     "dgmc_count_batch": (c_int, [c_int, c_int, P, c_float, P, c_size_t, P, P, P, P]),
     "dgmc_emit_batch": (c_int, [c_int, c_int, P, c_float, P, c_size_t, P, P, c_int64, P, c_int64, P]),

@@ -1401,6 +1401,137 @@ int dgmc_backward_batch(int B, int G, const int32_t* V_host, const float* phi, f
   return dgmc_backward_call("dgmc_backward_batch", B, G, V_host, phi, iso, vsrc, dL_dverts, dL_dphi, stream);
 }
 
+// dual marching cubes: the same conventions as dgmc_*, with dual vertices and quads in place of vertices and faces
+static int dgdmc_size(const char* fn, int B, int G, size_t* bytes) {
+  char msg[160];
+  if (B < 1 || B > dgm::MC_MAX_BATCH) {
+    snprintf(msg, sizeof(msg), "%s: B out of range (1 <= B <= 64)", fn);
+    return bad(msg);
+  }
+  if (G < 2 || G > 800 || !bytes) {
+    snprintf(msg, sizeof(msg), "%s: bad argument (2 <= G <= 800)", fn);
+    return bad(msg);
+  }
+  dgm::DmcWS::from(nullptr, G, B, bytes);
+  return DGM_OK;
+}
+
+int dgdmc_workspace_size(int G, size_t* bytes) { return dgdmc_size("dgdmc_workspace_size", 1, G, bytes); }
+int dgdmc_workspace_size_batch(int B, int G, size_t* bytes) {
+  return dgdmc_size("dgdmc_workspace_size_batch", B, G, bytes);
+}
+
+static int dgdmc_check(const char* fn, int B, int G, const float* phi, void* ws, size_t ws_bytes) {
+  char msg[160];
+  size_t need;
+  int rc = dgdmc_size(fn, B, G, &need);
+  if (rc != DGM_OK) return rc;
+  if (!phi || !ws) {
+    snprintf(msg, sizeof(msg), "%s: bad argument (null grid or workspace)", fn);
+    return bad(msg);
+  }
+  if (ws_bytes < need) {
+    snprintf(g_last_error, sizeof(g_last_error), "%s: workspace too small", fn);
+    return DGM_E_WORKSPACE;
+  }
+  return DGM_OK;
+}
+
+static int dgdmc_count_call(const char* fn, int B, int G, const float* phi, float iso, void* ws, size_t ws_bytes,
+                            int32_t* totals, int32_t* totals_host, void* totals_event, void* stream) {
+  int rc = dgdmc_check(fn, B, G, phi, ws, ws_bytes);
+  if (rc != DGM_OK) return rc;
+  if (!totals) {
+    char msg[160];
+    snprintf(msg, sizeof(msg), "%s: null totals", fn);
+    return bad(msg);
+  }
+  return check(dgm::launch_dmc_count(B, G, phi, iso, ws, totals, totals_host, (cudaEvent_t)totals_event,
+                                     (cudaStream_t)stream));
+}
+
+int dgdmc_count(int G, const float* phi, float iso, void* ws, size_t ws_bytes, int32_t* totals, int32_t* totals_host,
+                void* totals_event, void* stream) {
+  return dgdmc_count_call("dgdmc_count", 1, G, phi, iso, ws, ws_bytes, totals, totals_host, totals_event, stream);
+}
+
+int dgdmc_count_batch(int B, int G, const float* phi, float iso, void* ws, size_t ws_bytes, int32_t* totals,
+                      int32_t* totals_host, void* totals_event, void* stream) {
+  return dgdmc_count_call("dgdmc_count_batch", B, G, phi, iso, ws, ws_bytes, totals, totals_host, totals_event,
+                          stream);
+}
+
+static int dgdmc_emit_call(const char* fn, int B, int G, const float* phi, float iso, void* ws, size_t ws_bytes,
+                           float* verts, int32_t* vsrc, int64_t V_cap, int32_t* faces, int32_t* quads, int64_t Q_cap,
+                           void* stream) {
+  char msg[160];
+  if (V_cap < 0 || V_cap > dgm::DMC_MAX_VERTS || Q_cap < 0 || Q_cap > dgm::DMC_MAX_QUADS) {
+    snprintf(msg, sizeof(msg), "%s: capacity out of range (V_cap <= 2^28, Q_cap < 2^30)", fn);
+    return bad(msg);
+  }
+  if ((V_cap > 0 && (!verts || !vsrc)) || (Q_cap > 0 && !faces)) {
+    snprintf(msg, sizeof(msg), "%s: null output", fn);
+    return bad(msg);
+  }
+  int rc = dgdmc_check(fn, B, G, phi, ws, ws_bytes);
+  if (rc != DGM_OK) return rc;
+  return check(dgm::launch_dmc_emit(B, G, phi, iso, ws, verts, vsrc, V_cap, faces, quads, Q_cap,
+                                    (cudaStream_t)stream));
+}
+
+int dgdmc_emit(int G, const float* phi, float iso, void* ws, size_t ws_bytes, float* verts, int32_t* vsrc,
+               int64_t V_cap, int32_t* faces, int32_t* quads, int64_t Q_cap, void* stream) {
+  return dgdmc_emit_call("dgdmc_emit", 1, G, phi, iso, ws, ws_bytes, verts, vsrc, V_cap, faces, quads, Q_cap, stream);
+}
+
+int dgdmc_emit_batch(int B, int G, const float* phi, float iso, void* ws, size_t ws_bytes, float* verts,
+                     int32_t* vsrc, int64_t V_cap, int32_t* faces, int32_t* quads, int64_t Q_cap, void* stream) {
+  return dgdmc_emit_call("dgdmc_emit_batch", B, G, phi, iso, ws, ws_bytes, verts, vsrc, V_cap, faces, quads, Q_cap,
+                         stream);
+}
+
+static int dgdmc_backward_call(const char* fn, int B, int G, const int32_t* V_host, const float* phi, float iso,
+                               void* ws, size_t ws_bytes, const int32_t* vsrc, const float* dL_dverts,
+                               float* dL_dphi, void* stream) {
+  char msg[160];
+  int rc = dgdmc_check(fn, B, G, phi, ws, ws_bytes);
+  if (rc != DGM_OK) return rc;
+  if (!dL_dphi || !V_host) {
+    snprintf(msg, sizeof(msg), "%s: bad argument (null dL_dphi or V)", fn);
+    return bad(msg);
+  }
+  // each V_k comes from dgdmc_count: at most four dual vertices per cell, the batch within DMC_MAX_VERTS
+  const long long cells = 4ll * (G - 1) * (G - 1) * (G - 1);
+  dgm::McItems it;
+  it.B = B;
+  long long total = 0;
+  for (int k = 0; k < B; ++k) {
+    it.voff[k] = (int)total;
+    if (V_host[k] < 0 || V_host[k] > cells || total + V_host[k] > dgm::DMC_MAX_VERTS) {
+      snprintf(msg, sizeof(msg), "%s: V out of range", fn);
+      return bad(msg);
+    }
+    total += V_host[k];
+  }
+  it.voff[B] = (int)total;
+  if (total > 0 && (!vsrc || !dL_dverts)) {
+    snprintf(msg, sizeof(msg), "%s: null vsrc / dL_dverts", fn);
+    return bad(msg);
+  }
+  return check(dgm::launch_dmc_backward(G, it, phi, iso, ws, vsrc, dL_dverts, dL_dphi, (cudaStream_t)stream));
+}
+
+int dgdmc_backward(int G, int V, const float* phi, float iso, void* ws, size_t ws_bytes, const int32_t* vsrc,
+                   const float* dL_dverts, float* dL_dphi, void* stream) {
+  return dgdmc_backward_call("dgdmc_backward", 1, G, &V, phi, iso, ws, ws_bytes, vsrc, dL_dverts, dL_dphi, stream);
+}
+
+int dgdmc_backward_batch(int B, int G, const int32_t* V_host, const float* phi, float iso, void* ws, size_t ws_bytes,
+                         const int32_t* vsrc, const float* dL_dverts, float* dL_dphi, void* stream) {
+  return dgdmc_backward_call("dgdmc_backward_batch", B, G, V_host, phi, iso, ws, ws_bytes, vsrc, dL_dverts, dL_dphi,
+                             stream);
+}
+
 int dgl_gemm_ws_bytes(int M, int N, int K, size_t* bytes) {
   if (M <= 0 || N <= 0 || K <= 0 || !bytes) return bad("dgl_gemm_ws_bytes: bad argument");
   *bytes = dgm::gemm_test_ws_bytes(M, N > 256 ? N : 256, K);

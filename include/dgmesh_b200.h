@@ -892,6 +892,56 @@ int dgmc_backward_batch(int B, int G, const int32_t* V_host, const float* phi, f
                         const float* dL_dverts, float* dL_dphi, void* stream);
 
 /* ------------------------------------------------------------------------
+ * Differentiable dual marching cubes (Nielson 2004).  Stands in for diso.DiffDMC(grid, isovalue):
+ *   phi[G,G,G] fp32, iso  ->  verts[V,3] fp32 in [0,1]^3, faces[2Q,3] int32 and, optionally, quads[Q,4] int32
+ * Definition:
+ *   - A node is inside when phi < iso; corners, edges and case index are those of mc_tables.h.
+ *   - The patches of a case are the loops of tools/gen_mc_tables.py (DMC_PATCH, DMC_PATCH_OF_EDGE): at most 4
+ *     per case and 7 edges per patch; an ambiguous face separates the inside corners, as in marching cubes.
+ *   - A cut edge's crossing is marching cubes' vertex in grid units: t = (iso - p0)/(p1 - p0); pos = n;
+ *     pos[axis] += t.  A patch's dual vertex is the fp32 sum of its crossings in increasing edge id, divided by
+ *     its edge count, then by G - 1.  A patch gets a vertex only when one of its edges is interior (its four
+ *     incident cells lie in the grid), so no vertex is unreferenced.
+ *   - Every sign-changing interior edge gives one quad: the dual vertices of the four cells around it (each
+ *     cell's patch containing the edge) in cyclic order, oriented so the normal points from the inside node to
+ *     the outside one (as dgmc_*), starting at the lowest cell q0; triangles (q0,q1,q2), (q0,q2,q3).  Edges on
+ *     the grid's outer faces give nothing.  Q equals the number of interior marching-cubes vertices.
+ *   - Closed (every directed edge is matched by its reverse) but not always edge-manifold: in 36 ambiguous
+ *     (case, face) pairs one patch holds both segments of the face, and where the cells on both sides do that,
+ *     one dual edge is shared by four triangles.
+ *   - dL/dphi flows through each crossing's t with weight 1/k per crossing of a k-edge patch; nothing flows to
+ *     iso.  The backward gathers the <= 24 (cell, patch) terms of every node in a fixed order, without float
+ *     atomics: its result is bit-identical from run to run.
+ * Calls, as dgmc_*: dgdmc_count writes totals[2] = {V, Q} (and the same pair to totals_host behind
+ * totals_event); dgdmc_emit writes up to V_cap vertices (verts, and vsrc[V_cap] = cell * 4 + patch, which the
+ * backward reads) and up to Q_cap quads (faces[2 Q_cap, 3]; quads[Q_cap, 4] when not NULL), capacities enforced
+ * on the device, so it may be enqueued optimistically and re-run when something did not fit.
+ * Limits: 2 <= G <= 800; V is at most 4 (G-1)^3 and Q at most 3 G^2 (G-1); V_cap <= 2^28 (a cell's first
+ * vertex and cell * 4 + patch are packed into 32-bit records), Q_cap < 2^30 (2 Q triangles < 2^31).
+ * dgdmc_backward: dL_dverts[V,3] -> dL_dphi[G,G,G] (fully written), V as returned by dgdmc_count, vsrc as
+ * written by dgdmc_emit; it takes a workspace of dgdmc_workspace_size bytes, which need not be the forward's.
+ * The _batch forms take B grids phi[B,G,G,G], 1 <= B <= 64, with the layout of dgmc_*_batch: item k's
+ * vertices and quads follow those of items 0..k-1, indices local to the item, and item k's slice is exactly
+ * what the single call gives for grid k; V_host[B] are the items' vertex counts.  The workspace holds the
+ * brick totals and an 8-byte record per cell: about 191 MB per item at G = 288.  Bad arguments are refused on
+ * the host before any device work.
+ * ------------------------------------------------------------------------ */
+int dgdmc_workspace_size(int G, size_t* bytes);
+int dgdmc_workspace_size_batch(int B, int G, size_t* bytes);
+int dgdmc_count(int G, const float* phi, float iso, void* ws, size_t ws_bytes,
+                int32_t* totals, int32_t* totals_host, void* totals_event, void* stream);
+int dgdmc_count_batch(int B, int G, const float* phi, float iso, void* ws, size_t ws_bytes,
+                      int32_t* totals, int32_t* totals_host, void* totals_event, void* stream);
+int dgdmc_emit(int G, const float* phi, float iso, void* ws, size_t ws_bytes, float* verts, int32_t* vsrc,
+               int64_t V_cap, int32_t* faces, int32_t* quads, int64_t Q_cap, void* stream);
+int dgdmc_emit_batch(int B, int G, const float* phi, float iso, void* ws, size_t ws_bytes, float* verts,
+                     int32_t* vsrc, int64_t V_cap, int32_t* faces, int32_t* quads, int64_t Q_cap, void* stream);
+int dgdmc_backward(int G, int V, const float* phi, float iso, void* ws, size_t ws_bytes, const int32_t* vsrc,
+                   const float* dL_dverts, float* dL_dphi, void* stream);
+int dgdmc_backward_batch(int B, int G, const int32_t* V_host, const float* phi, float iso, void* ws, size_t ws_bytes,
+                         const int32_t* vsrc, const float* dL_dverts, float* dL_dphi, void* stream);
+
+/* ------------------------------------------------------------------------
  * Tensor-core GEMM building blocks of the MLPs (wgmma, bf16 operands, fp32 accumulation in
  * registers), exposed stand-alone for the parity tests (torch.matmul on the same bf16 operands is the
  * oracle).  The networks below drive the same two kernels on activations kept in the library's

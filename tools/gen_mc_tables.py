@@ -14,7 +14,9 @@ consulted.  Instead of typing a table from memory, the cases are DERIVED here:
     and each loop is fan-triangulated, oriented so the normal points from inside to outside.
 
 Output: dg-mesh_b200/csrc/mc_tables.h with  MC_NTRI[256]  and  MC_TRI[256][MC_MAX_TRI*3]
-(edge ids, -1 padded).  `python tools/gen_mc_tables.py --check` verifies the committed header.
+(edge ids, -1 padded), and the dual-marching-cubes patches of the same loops: DMC_PATCH[256][4][7] (each
+patch's edges in increasing id, -1 padded) and DMC_PATCH_OF_EDGE[256][12] (-1 for an edge the level set does
+not cut).  `python tools/gen_mc_tables.py --check` verifies the committed header.
 """
 import itertools
 import os
@@ -64,7 +66,10 @@ def faces():
 FACES = faces()
 
 
-def case_triangles(case):
+def case_loops(case):
+    """The closed loops of intersected edges of a case, each oriented so that its normal points from inside to
+    outside.  A loop is one surface patch of the cell: the triangles of case_triangles and the patches of dual
+    marching cubes are both built from these loops."""
     inside = [(case >> v) & 1 for v in range(8)]
     segs = []
     for cyc in FACES:
@@ -101,7 +106,7 @@ def case_triangles(case):
             seen.add(n)
             prev, cur = cur, n
         loops.append(loop)
-    tris = []
+    out = []
     mid = lambda e: (corner_xyz(EDGES[e][0]) + corner_xyz(EDGES[e][1])) / 2.0  # noqa: E731
     for loop in loops:
         pts = np.array([mid(e) for e in loop])
@@ -116,15 +121,56 @@ def case_triangles(case):
             d += (corner_xyz(b) - corner_xyz(a)) * (1 if ia else -1) if ia != ib else 0
         if np.dot(nrm, d) < 0:
             loop = loop[::-1]
+        out.append(loop)
+    return out
+
+
+def case_triangles(case):
+    tris = []
+    for loop in case_loops(case):
         for i in range(1, len(loop) - 1):
             tris.append((loop[0], loop[i], loop[i + 1]))
     return tris
+
+
+def case_patches(case):
+    """Dual marching cubes: the patches of a case, one per loop, each as its edges in increasing edge id (the
+    order in which a dual vertex sums its crossings)."""
+    return [sorted(loop) for loop in case_loops(case)]
 
 
 def build():
     table = [case_triangles(c) for c in range(256)]
     mx = max(len(t) for t in table)
     return table, mx
+
+
+def patch_tables():
+    """(patch[256, DMC_MAX_PATCH, DMC_MAX_PATCH_EDGES], patch_of_edge[256, 12]), -1 padded."""
+    pt = [case_patches(c) for c in range(256)]
+    mp, me = max(len(p) for p in pt), max(len(q) for p in pt for q in p)
+    assert (mp, me) == (4, 7), (mp, me)
+    patch = -np.ones((256, mp, me), np.int64)
+    pof = -np.ones((256, 12), np.int64)
+    for c, ps in enumerate(pt):
+        for i, q in enumerate(ps):
+            patch[c, i, :len(q)] = q
+            pof[c, q] = i
+    return patch, pof
+
+
+def render_patches():
+    patch, pof = patch_tables()
+    lines = ["// Dual marching cubes: patch p of a case is one loop above, as its edges in increasing id.",
+             f"#define DMC_MAX_PATCH {patch.shape[1]}", f"#define DMC_MAX_PATCH_EDGES {patch.shape[2]}",
+             f"static const signed char DMC_PATCH[256][{patch.shape[1]}][{patch.shape[2]}] = {{"]
+    for c in range(256):
+        lines.append("    {" + ", ".join("{" + ", ".join(f"{v:2d}" for v in q) + "}" for q in patch[c]) + "},")
+    lines += ["};", "static const signed char DMC_PATCH_OF_EDGE[256][12] = {"]
+    for c in range(256):
+        lines.append("    {" + ", ".join(f"{v:2d}" for v in pof[c]) + "},")
+    lines.append("};")
+    return "\n".join(lines) + "\n"
 
 
 def render(table, mx):
@@ -143,7 +189,7 @@ def render(table, mx):
         flat += [-1] * (mx * 3 - len(flat))
         lines.append("    {" + ", ".join(f"{v:2d}" for v in flat) + "},")
     lines.append("};")
-    return "\n".join(lines) + "\n"
+    return "\n".join(lines) + "\n" + render_patches()
 
 
 def tables_for_python():
@@ -154,6 +200,12 @@ def tables_for_python():
         flat = [e for x in t for e in x]
         tri[c, :len(flat)] = flat
     return np.array([len(t) for t in table]), tri, np.array([EDGES[e][0] for e in range(12)])
+
+
+def dmc_tables_for_python():
+    """(patch[256, 4, 7], patch_of_edge[256, 12], edge_lo[12]) for the dual-marching-cubes reference."""
+    patch, pof = patch_tables()
+    return patch, pof, np.array([EDGES[e][0] for e in range(12)])
 
 
 if __name__ == "__main__":
