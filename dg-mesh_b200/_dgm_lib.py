@@ -281,6 +281,15 @@ SIGNATURES.update({
     "dghp_reg_backward": (c_int, _HP_HEAD[2:] + [P, P, P, P]),
 })
 
+# hash-grid field: (F, N, G, grids_host, L, Fe, log2_table, res_host, R_t) + forward: box, x, t, tables_host, out /
+# backward: box, x, t, tables_host, grad_out, grad_x, grad_tables_host, ws, bytes; + stream
+_HG_HEAD = [c_int, c_int, c_int, P, c_int, c_int, c_int, P, c_int]
+SIGNATURES.update({
+    "dghg_forward": (c_int, _HG_HEAD + [P, P, P, P, P, P]),
+    "dghg_backward_workspace": (c_int, _HG_HEAD + [ctypes.POINTER(c_size_t)]),
+    "dghg_backward": (c_int, _HG_HEAD + [P, P, P, P, P, P, P, P, c_size_t, P]),
+})
+
 KERNEL_NAMES = ["preprocess", "tile_scan", "scatter", "sort_pack", "render_fwd", "render_bwd", "preprocess_bwd",
                 "count", "normal_grad_finish", "median_grad", "feature_fwd", "feature_bwd", "feature_grad_finish",
                 "blend_stats"]

@@ -16,6 +16,7 @@
 #include "mesh_distance_kernels.h"
 #include "deform_reg_kernels.h"
 #include "hexplane_kernels.h"
+#include "hashgrid_kernels.h"
 #include "meshrast_kernels.h"
 #include "nvls_kernels.h"
 
@@ -2411,6 +2412,111 @@ int dghp_reg_backward(int S, int C, const int32_t* res_host, int R_t, const floa
   if (rc != DGM_OK) return rc;
   if (!grad_losses) return bad("dghp_reg_backward: null pointer");
   return check(dgm::launch_hexplane_reg_bwd(f, grad_losses, g, (cudaStream_t)stream));
+}
+
+// ---- hash-grid field.  Every argument is checked here, before any device work.
+namespace {
+// the field's shape (kinds, resolutions, dense levels) and, when tables_host is given, its G table pointers
+int dghg_args(const char* fn, int F, int N, int G, const int32_t* grids_host, int L, int Fe, int log2_table,
+              const int32_t* res_host, int R_t, const float* const* tables_host, dgm::HgField& f) {
+  char msg[200];
+  if (G < 1 || G > HG_MAX_G || L < 1 || L > HG_MAX_L || (Fe != 2 && Fe != 4) || log2_table < 12 || log2_table > 24 ||
+      R_t < 1) {
+    snprintf(msg, sizeof(msg), "%s: bad size (1 <= G <= 4, 1 <= L <= 24, Fe = 2 or 4, 12 <= log2_table <= 24, R_t >= 1)",
+             fn);
+    return bad(msg);
+  }
+  if (!grids_host || !res_host) {
+    snprintf(msg, sizeof(msg), "%s: null pointer (%s)", fn, grids_host ? "res_host" : "grids_host");
+    return bad(msg);
+  }
+  const int64_t T = (int64_t)1 << log2_table, GLFe = (int64_t)G * L * Fe;
+  if (F < 0 || N < 0 || (int64_t)L * T * Fe >= ((int64_t)1 << 31) || (int64_t)F * N * GLFe >= ((int64_t)1 << 31) ||
+      (int64_t)N * F >= ((int64_t)1 << 31)) {
+    snprintf(msg, sizeof(msg), "%s: bad size (F, N >= 0; L T Fe, F N G L Fe and N F < 2^31)", fn);
+    return bad(msg);
+  }
+  memset(&f, 0, sizeof(f));
+  f.G = G, f.L = L, f.Fe = Fe, f.log2T = log2_table;
+  for (int g = 0; g < G; ++g) {
+    if (grids_host[g] < 0 || grids_host[g] > 3 || (g > 0 && grids_host[g] <= grids_host[g - 1])) {
+      snprintf(msg, sizeof(msg), "%s: bad grids (kinds 0 xyz, 1 xyt, 2 yzt, 3 xzt, strictly increasing)", fn);
+      return bad(msg);
+    }
+    f.kind[g] = grids_host[g];
+  }
+  for (int l = 0; l < L; ++l) {
+    if (res_host[l] < 1 || res_host[l] > (1 << 24)) {
+      snprintf(msg, sizeof(msg), "%s: bad size (level resolutions in [1, 2^24])", fn);
+      return bad(msg);
+    }
+    f.R[l] = res_host[l];
+    f.Rt[l] = res_host[l] < R_t ? res_host[l] : R_t;
+  }
+  for (int g = 0; g < G; ++g)
+    for (int l = 0; l < L; ++l) {
+      const int64_t r = f.R[l] + 1, rc = (f.kind[g] == 0 ? f.R[l] : f.Rt[l]) + 1;
+      if (r * r * rc <= T) f.dense[g] |= 1u << l;
+    }
+  if (!tables_host) return DGM_OK;
+  for (int g = 0; g < G; ++g) {
+    if (!tables_host[g]) {
+      snprintf(msg, sizeof(msg), "%s: null pointer (table %d)", fn, g);
+      return bad(msg);
+    }
+    f.tab[g] = tables_host[g];
+  }
+  return DGM_OK;
+}
+
+bool dghg_timed(const dgm::HgField& f) { return f.kind[f.G - 1] != 0; }
+}  // namespace
+
+int dghg_forward(int F, int N, int G, const int32_t* grids_host, int L, int Fe, int log2_table,
+                 const int32_t* res_host, int R_t, const float* box, const float* x, const float* t,
+                 const float* const* tables_host, float* out, void* stream) {
+  dgm::HgField f;
+  if (!tables_host) return bad("dghg_forward: null pointer");
+  const int rc = dghg_args("dghg_forward", F, N, G, grids_host, L, Fe, log2_table, res_host, R_t, tables_host, f);
+  if (rc != DGM_OK) return rc;
+  if (F == 0 || N == 0) return DGM_OK;
+  if (!box || !x || (!t && dghg_timed(f)) || !out) return bad("dghg_forward: null pointer");
+  return check(dgm::launch_hashgrid_fwd(F, N, f, box, x, t, out, (cudaStream_t)stream));
+}
+
+int dghg_backward_workspace(int F, int N, int G, const int32_t* grids_host, int L, int Fe, int log2_table,
+                            const int32_t* res_host, int R_t, size_t* bytes) {
+  dgm::HgField f;
+  const int rc = dghg_args("dghg_backward_workspace", F, N, G, grids_host, L, Fe, log2_table, res_host, R_t, nullptr, f);
+  if (rc != DGM_OK) return rc;
+  if (!bytes) return bad("dghg_backward_workspace: null pointer");
+  *bytes = dgm::hg_ws_bytes(f);
+  return DGM_OK;
+}
+
+int dghg_backward(int F, int N, int G, const int32_t* grids_host, int L, int Fe, int log2_table,
+                  const int32_t* res_host, int R_t, const float* box, const float* x, const float* t,
+                  const float* const* tables_host, const float* grad_out, float* grad_x,
+                  float* const* grad_tables_host, void* ws, size_t ws_bytes, void* stream) {
+  dgm::HgField f;
+  dgm::HgGrads g;
+  if (!tables_host || !grad_tables_host) return bad("dghg_backward: null pointer");
+  const int rc = dghg_args("dghg_backward", F, N, G, grids_host, L, Fe, log2_table, res_host, R_t, tables_host, f);
+  if (rc != DGM_OK) return rc;
+  for (int i = 0; i < G; ++i) {
+    if (!grad_tables_host[i]) {
+      char msg[200];
+      snprintf(msg, sizeof(msg), "dghg_backward: null pointer (table gradient %d)", i);
+      return bad(msg);
+    }
+    g.tab[i] = grad_tables_host[i];
+  }
+  if (F > 0 && N > 0) {
+    if (!box || !x || (!t && dghg_timed(f)) || !grad_out || !ws) return bad("dghg_backward: null pointer");
+    const size_t need = dgm::hg_ws_bytes(f);
+    if (ws_bytes < need) return dge_short("dghg_backward", ws_bytes, need);
+  }
+  return check(dgm::launch_hashgrid_bwd(F, N, f, box, x, t, grad_out, grad_x, g, ws, (cudaStream_t)stream));
 }
 
 // ---- early notification objects: an event + a device-mapped pinned status mirror.  These are the

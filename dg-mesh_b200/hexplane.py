@@ -216,22 +216,18 @@ class HexPlaneField(nn.Module):
         return _RegFn.apply(self._shape, *self.planes)
 
 
-class HexPlaneDeformNetwork(nn.Module):
-    """4D-GS's deformation network over a HexPlaneField, shaped like utils.time_utils.DeformNetwork:
-    forward(x, t) -> (d_xyz, d_rotation, d_scaling), or with normal=True (d_xyz, d_rotation, d_scaling, d_normal) as
-    DeformNetworkNormal returns.  The field is followed by Linear(S C, W) and one head per output:
-    ReLU -> Linear(W, W) -> ReLU -> Linear(W, rows).  With t [F,N,1] every output is [F,N,rows] (the per-frame
-    deltas render_batch takes), the spatial planes sampled once per point for the whole batch.
-
-    field_kw goes to HexPlaneField (channels, base_resolution, multires, time_resolution).  The heads are plain
-    nn.Linear; every parameter is an ordinary nn.Parameter (optim.FusedAdam and state_dict work unchanged)."""
+class DeformHeads(nn.Module):
+    """4D-GS's deformation heads over a feature field (`field(x, t)` -> [..., field.out_dim]), shaped like
+    utils.time_utils.DeformNetwork: forward(x, t) -> (d_xyz, d_rotation, d_scaling), or with normal=True
+    (d_xyz, d_rotation, d_scaling, d_normal) as DeformNetworkNormal returns.  The field is followed by
+    Linear(out_dim, W) and one head per output: ReLU -> Linear(W, W) -> ReLU -> Linear(W, rows).  The field is
+    registered first, so parameter order and state_dict keys are field.*, feature_out.*, then the heads."""
     HEADS = (("gaussian_warp", 3), ("gaussian_rotation", 4), ("gaussian_scaling", 3))
 
-    def __init__(self, box, normal=False, W=64, **field_kw):
+    def __init__(self, field, normal, W):
         super().__init__()
-        _int("HexPlaneDeformNetwork", "W", W, 1)
-        self.field = HexPlaneField(box, **field_kw)
-        self.feature_out = nn.Linear(self.field.out_dim, W)
+        self.field = field
+        self.feature_out = nn.Linear(field.out_dim, W)
         self.heads = self.HEADS + ((("gaussian_normal", 3),) if normal else ())
         for name, rows in self.heads:
             setattr(self, name, nn.Sequential(nn.ReLU(), nn.Linear(W, W), nn.ReLU(), nn.Linear(W, rows)))
@@ -239,3 +235,18 @@ class HexPlaneDeformNetwork(nn.Module):
     def forward(self, x, t):
         h = self.feature_out(self.field(x, t))
         return tuple(getattr(self, name)(h) for name, _ in self.heads)
+
+
+class HexPlaneDeformNetwork(DeformHeads):
+    """4D-GS's deformation network over a HexPlaneField (the DeformHeads on it), shaped like
+    utils.time_utils.DeformNetwork: forward(x, t) -> (d_xyz, d_rotation, d_scaling), or with normal=True
+    (d_xyz, d_rotation, d_scaling, d_normal) as DeformNetworkNormal returns.  With t [F,N,1] every output is
+    [F,N,rows] (the per-frame deltas render_batch takes), the spatial planes sampled once per point for the whole
+    batch.
+
+    field_kw goes to HexPlaneField (channels, base_resolution, multires, time_resolution).  The heads are plain
+    nn.Linear; every parameter is an ordinary nn.Parameter (optim.FusedAdam and state_dict work unchanged)."""
+
+    def __init__(self, box, normal=False, W=64, **field_kw):
+        _int("HexPlaneDeformNetwork", "W", W, 1)
+        super().__init__(HexPlaneField(box, **field_kw), normal, W)

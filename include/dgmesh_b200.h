@@ -1482,6 +1482,45 @@ int dghp_reg_forward(int S, int C, const int32_t* res_host, int R_t, const float
 int dghp_reg_backward(int S, int C, const int32_t* res_host, int R_t, const float* const* planes_host,
                       const float* grad_losses, float* const* grad_planes_host, void* stream);
 
+/* ------------------------------------------------------------------------
+ * Multiresolution hash-grid field of (x, y, z, t) (Instant-NGP's HashGrid; Grid4D's space-time grids).  Device
+ * pointers, except grids_host [G], res_host [L], tables_host and grad_tables_host [G] (host arrays).  Nothing
+ * allocates or synchronises with the host.  DGM_E_BADARG before any device work for: G outside [1, 4], L outside
+ * [1, 24], Fe not 2 or 4, log2_table outside [12, 24], R_t < 1, a level resolution outside [1, 2^24], grids_host
+ * not strictly increasing kinds in [0, 3], F < 0, N < 0, L T Fe >= 2^31, F N G L Fe >= 2^31, N F >= 2^31, or a NULL
+ * pointer (t may be NULL when no grid uses time); a workspace below its query: DGM_E_WORKSPACE.  F = 0 or N = 0
+ * writes nothing (the backward zeroes the table gradients).
+ *
+ * The field: x [N,3] canonical positions, t [F,N] times, box [6] = (lo xyz, hi xyz) device floats.  Grid g is of
+ * kind grids_host[g]: 0 = xyz, 1 = xyt, 2 = yzt, 3 = xzt, its three axes the coordinates the name spells, in order.
+ * Its table tables_host[g] is [L, T, Fe] float32, T = 2^log2_table.  In float32, exactly as written (no fast math):
+ *   u = (x - lo) / (hi - lo) per spatial axis, u = t on the time axis, then u = min(max(u, 0), 1);
+ *   per axis of level l, with R = res_host[l] (spatial) or min(res_host[l], R_t) (time):
+ *     p = u R (one rounded product), c = min(floor(p), R - 1), w = p - c (exact; 1 on the top face);
+ *   the 8 nodes c + {0,1}^3 have slots
+ *     dense level, (R_a + 1)(R_b + 1)(R_c + 1) <= T: i_a + (R_a + 1) (i_b + (R_b + 1) i_c)   (first axis fastest)
+ *     hashed level, otherwise:  (i_a * 1 ^ i_b * 2654435761 ^ i_c * 805459861) mod T        (uint32 wrap-around)
+ *   out[f, n, (g L + l) Fe + e] = sum over the 8 nodes of the trilinear weight times table_g[l, slot, e]
+ *   (out [F,N,G L Fe]: grid, then level, then feature; the spatial grid is the same in every frame).
+ * dghg_forward keeps nothing for the backward.
+ * dghg_backward: grad_out [F,N,G L Fe] -> grad_x [N,3] (NULL: not computed) and every table's gradient
+ *   (grad_tables_host, each written, not accumulated; a dense level's unused slots are 0).  dL/dx passes through each
+ *   grid's spatial axes and is 0 where the unclamped u is outside [0, 1] (it passes at u = 0 and u = 1, as
+ *   torch.clamp); t takes none.  The table gradients are sums in int64 fixed point at a power-of-two scale chosen
+ *   per (grid, level) from max |grad_out|, so they are bit-identical from run to run; a non-finite grad_out in a
+ *   (grid, level) makes that level's table gradient NaN.  Workspace: dghg_backward_workspace (G L T Fe 8 bytes and
+ *   a little more; independent of F and N).
+ * ------------------------------------------------------------------------ */
+int dghg_forward(int F, int N, int G, const int32_t* grids_host, int L, int Fe, int log2_table,
+                 const int32_t* res_host, int R_t, const float* box, const float* x, const float* t,
+                 const float* const* tables_host, float* out, void* stream);
+int dghg_backward_workspace(int F, int N, int G, const int32_t* grids_host, int L, int Fe, int log2_table,
+                            const int32_t* res_host, int R_t, size_t* bytes);
+int dghg_backward(int F, int N, int G, const int32_t* grids_host, int L, int Fe, int log2_table,
+                  const int32_t* res_host, int R_t, const float* box, const float* x, const float* t,
+                  const float* const* tables_host, const float* grad_out, float* grad_x,
+                  float* const* grad_tables_host, void* ws, size_t ws_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
