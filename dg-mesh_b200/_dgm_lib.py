@@ -100,6 +100,11 @@ SIGNATURES = {
     "dgdmc_emit_batch": (c_int, [c_int, c_int, P, c_float, P, c_size_t, P, P, c_int64, P, P, c_int64, P]),
     "dgdmc_backward": (c_int, [c_int, c_int, P, c_float, P, c_size_t, P, P, P, P]),
     "dgdmc_backward_batch": (c_int, [c_int, c_int, P, P, c_float, P, c_size_t, P, P, P, P]),
+    "dgfc_emit": (c_int, [c_int, P, c_float, P, P, P, P, c_int, c_int, P, c_size_t, P, P, P, P, c_int64, P, P,
+                          c_int64, P]),
+    "dgfc_backward_workspace_size": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "dgfc_backward": (c_int, [c_int, c_int, c_int, P, c_float, P, P, P, P, c_int, c_int, P, P, P, P, P, P, c_size_t,
+                              P, P, P, P, P, P]),
     "dgmc_workspace_size_batch": (c_int, [c_int, c_int, ctypes.POINTER(c_size_t)]),
     "dgmc_count_batch": (c_int, [c_int, c_int, P, c_float, P, c_size_t, P, P, P, P]),
     "dgmc_emit_batch": (c_int, [c_int, c_int, P, c_float, P, c_size_t, P, P, c_int64, P, c_int64, P]),

@@ -6,6 +6,7 @@
 #include "knn_kernels.h"
 #include "dpsr_kernels.h"
 #include "mc_kernels.h"
+#include "flexicubes_kernels.h"
 #include "loss_kernels.h"
 #include "mlp_kernels.h"
 #include "densify_kernels.h"
@@ -1531,6 +1532,96 @@ int dgdmc_backward_batch(int B, int G, const int32_t* V_host, const float* phi, 
                          const int32_t* vsrc, const float* dL_dverts, float* dL_dphi, void* stream) {
   return dgdmc_backward_call("dgdmc_backward_batch", B, G, V_host, phi, iso, ws, ws_bytes, vsrc, dL_dverts, dL_dphi,
                              stream);
+}
+
+// FlexiCubes: dual marching cubes' count (dgdmc_count) and workspace, with weighted crossings and vertices, node
+// offsets and the gamma split
+static int dgfc_weights(const char* fn, const float* alpha, const float* beta, const float* gamma_f, int training,
+                        const float* dalpha, const float* dbeta, const float* dgamma) {
+  char msg[160];
+  if ((dalpha && !alpha) || (dbeta && !beta) || (dgamma && !gamma_f)) {
+    snprintf(msg, sizeof(msg), "%s: a gradient was requested for a null weight", fn);
+    return bad(msg);
+  }
+  if (dgamma && !training) {
+    snprintf(msg, sizeof(msg), "%s: dL_dgamma is only defined in training mode", fn);
+    return bad(msg);
+  }
+  return DGM_OK;
+}
+
+int dgfc_emit(int G, const float* phi, float iso, const float* deform, const float* alpha, const float* beta,
+              const float* gamma_f, int training, int normalize, void* ws, size_t ws_bytes, float* verts,
+              int32_t* vsrc, float* ldev, int32_t* vk, int64_t V_cap, int32_t* faces, int32_t* quads, int64_t Q_cap,
+              void* stream) {
+  const char* fn = "dgfc_emit";
+  char msg[160];
+  const long long q_max = training ? dgm::FC_MAX_QUADS_TRAINING : dgm::DMC_MAX_QUADS;
+  if (V_cap < 0 || V_cap > dgm::DMC_MAX_VERTS || Q_cap < 0 || Q_cap > q_max) {
+    snprintf(msg, sizeof(msg), "%s: capacity out of range (V_cap <= 2^28, Q_cap < 2^30, < 2^29 in training)", fn);
+    return bad(msg);
+  }
+  if ((V_cap > 0 && (!verts || !vsrc || !ldev || !vk)) || (Q_cap > 0 && (!faces || !quads))) {
+    snprintf(msg, sizeof(msg), "%s: null output", fn);
+    return bad(msg);
+  }
+  int rc = dgdmc_check(fn, 1, G, phi, ws, ws_bytes);
+  if (rc != DGM_OK) return rc;
+  const dgm::FcParams w{deform, alpha, beta, gamma_f};
+  return check(dgm::launch_fc_emit(G, phi, iso, w, training != 0, normalize != 0, ws, verts, vsrc, ldev, vk, V_cap,
+                                   faces, quads, Q_cap, (cudaStream_t)stream));
+}
+
+static int dgfc_counts(const char* fn, int G, int V, int Q, int training) {
+  char msg[160];
+  const long long G1 = G - 1;
+  const long long q_max = training ? dgm::FC_MAX_QUADS_TRAINING : dgm::DMC_MAX_QUADS;
+  if (G < 2 || G > 800) {
+    snprintf(msg, sizeof(msg), "%s: bad argument (2 <= G <= 800)", fn);
+    return bad(msg);
+  }
+  if (V < 0 || V > 4 * G1 * G1 * G1 || V > dgm::DMC_MAX_VERTS || Q < 0 || Q > 3ll * G * G * G1 || Q > q_max) {
+    snprintf(msg, sizeof(msg), "%s: V or Q out of range", fn);
+    return bad(msg);
+  }
+  return DGM_OK;
+}
+
+int dgfc_backward_workspace_size(int G, int V, int Q, int training, size_t* bytes) {
+  int rc = dgfc_counts("dgfc_backward_workspace_size", G, V, Q, training);
+  if (rc != DGM_OK) return rc;
+  if (!bytes) return bad("dgfc_backward_workspace_size: null bytes");
+  *bytes = dgm::fc_backward_ws_bytes(G, V, Q, training != 0);
+  return DGM_OK;
+}
+
+int dgfc_backward(int G, int V, int Q, const float* phi, float iso, const float* deform, const float* alpha,
+                  const float* beta, const float* gamma_f, int training, int normalize, const float* verts,
+                  const int32_t* vsrc, const int32_t* quads, const float* dL_dverts, const float* dL_dldev, void* ws,
+                  size_t ws_bytes, float* dL_dphi, float* dL_ddeform, float* dL_dalpha, float* dL_dbeta,
+                  float* dL_dgamma, void* stream) {
+  const char* fn = "dgfc_backward";
+  char msg[160];
+  int rc = dgfc_counts(fn, G, V, Q, training);
+  if (rc != DGM_OK) return rc;
+  if (!phi || !ws || !dL_dphi || (dL_ddeform && !deform)) {
+    snprintf(msg, sizeof(msg), "%s: bad argument (null grid, workspace or dL_dphi, or dL_ddeform without deform)", fn);
+    return bad(msg);
+  }
+  rc = dgfc_weights(fn, alpha, beta, gamma_f, training, dL_dalpha, dL_dbeta, dL_dgamma);
+  if (rc != DGM_OK) return rc;
+  if ((V > 0 && (!vsrc || !dL_dverts)) || (training && V > 0 && !verts) || (training && Q > 0 && !quads)) {
+    snprintf(msg, sizeof(msg), "%s: null verts / vsrc / quads / dL_dverts", fn);
+    return bad(msg);
+  }
+  if (ws_bytes < dgm::fc_backward_ws_bytes(G, V, Q, training != 0)) {
+    snprintf(g_last_error, sizeof(g_last_error), "%s: workspace too small", fn);
+    return DGM_E_WORKSPACE;
+  }
+  const dgm::FcParams w{deform, alpha, beta, gamma_f};
+  return check(dgm::launch_fc_backward(G, V, Q, phi, iso, w, training != 0, normalize != 0, verts, vsrc, quads,
+                                       dL_dverts, dL_dldev, ws, dL_dphi, dL_ddeform, dL_dalpha, dL_dbeta, dL_dgamma,
+                                       (cudaStream_t)stream));
 }
 
 int dgl_gemm_ws_bytes(int M, int N, int K, size_t* bytes) {

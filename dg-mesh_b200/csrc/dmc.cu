@@ -14,44 +14,11 @@
 // Backward: vsrc rebuilds every cell's first vertex; then one thread per NODE gathers, in a fixed order, the
 // <= 24 (cell, patch) terms of its six edges: the gradient is bit-identical from run to run, no float atomics.
 #include "common.cuh"
+#include "dmc_cell.cuh"
 #include "mc_kernels.h"
 #include "mc_sweep.cuh"
-#include "mc_tables.h"
 
 namespace dgm {
-
-// per case, built from DMC_PATCH_OF_EDGE: the patch of every edge as 12 nibbles (15: the edge is not cut), and
-// the 12-bit edge mask of each patch at bits 16 p
-__device__ unsigned long long g_dmc_pof[256];
-__device__ unsigned long long g_dmc_pmask[256];
-
-// bit e: edge e of cell (i, j, k) is interior -- its two coordinates across the edge, cell + combo bit, lie in
-// [1, G - 2].  Edge e = 4 * axis + combo, combo bit 0 / 1 for the lower / higher of the other two axes.
-__device__ __forceinline__ unsigned dmc_interior_edges(int G, int i, int j, int k) {
-  const bool lo0 = i >= 1, lo1 = j >= 1, lo2 = k >= 1, hi0 = i <= G - 3, hi1 = j <= G - 3, hi2 = k <= G - 3;
-  unsigned m = 0;
-#pragma unroll
-  for (int e = 0; e < 12; ++e) {
-    const int a = e >> 2;
-    const bool b0 = a == 0 ? ((e & 1) ? hi1 : lo1) : ((e & 1) ? hi0 : lo0);
-    const bool b1 = a == 2 ? ((e & 2) ? hi1 : lo1) : ((e & 2) ? hi2 : lo2);
-    m |= (unsigned)(b0 && b1) << e;
-  }
-  return m;
-}
-
-// the patches of case cs with a dual vertex: those with an interior edge
-__device__ __forceinline__ unsigned dmc_need(unsigned long long pm, unsigned imask) {
-  unsigned need = 0;
-#pragma unroll
-  for (int p = 0; p < 4; ++p) need |= (unsigned)((((unsigned)(pm >> (16 * p))) & imask & 0xfffu) != 0) << p;
-  return need;
-}
-
-// the cut edges of a case (union of its patches)
-__device__ __forceinline__ unsigned dmc_cut(unsigned long long pm) {
-  return (unsigned)(pm | (pm >> 16) | (pm >> 32) | (pm >> 48)) & 0xfffu;
-}
 
 // quads a cell owns: its cut interior edges 3, 7, 11 (the x, y and z edges through corner 7)
 #define DMC_QUAD_EDGES 0x888u
@@ -186,14 +153,6 @@ __global__ void __launch_bounds__(32 * MC_WARPS) dmc_emit_kernel(
       }
     }
   }
-}
-
-// dual vertex (item-local) of the patch of cell `c` (cell coordinates ci, cj, ck) that contains local edge le
-__device__ __forceinline__ uint32_t dmc_vertex_of(int G, unsigned long long w, int ci, int cj, int ck, int le) {
-  const unsigned cs = (unsigned)(w >> 32) & 255u;
-  const unsigned p = (unsigned)(__ldg(&g_dmc_pof[cs]) >> (4 * le)) & 15u;
-  const unsigned need = dmc_need(__ldg(&g_dmc_pmask[cs]), dmc_interior_edges(G, ci, cj, ck));
-  return (uint32_t)w + (uint32_t)__popc(need & ((1u << p) - 1u));
 }
 
 // one thread per quad: the reference lowest cell * 3 + axis a -> the four cells around the edge through that
@@ -358,27 +317,6 @@ __global__ void __launch_bounds__(256) dmc_backward_kernel(int G, McItems it, co
   dphi[x] = acc;
 }
 
-static unsigned long long g_dmc_tables_uploaded = 0;  // per device
-static cudaError_t upload_dmc_tables() {
-  if (!once_per_device(g_dmc_tables_uploaded)) return cudaSuccess;
-  unsigned long long pof[256], pmask[256];
-  for (int cs = 0; cs < 256; ++cs) {
-    pof[cs] = ~0ull;
-    pmask[cs] = 0;
-    for (int e = 0; e < 12; ++e) {
-      const int p = DMC_PATCH_OF_EDGE[cs][e];
-      if (p >= 0) {
-        pof[cs] &= ~(15ull << (4 * e)) | ((unsigned long long)p << (4 * e));
-        pmask[cs] |= 1ull << (16 * p + e);
-      }
-    }
-  }
-  cudaError_t e = cudaMemcpyToSymbol(g_dmc_pof, pof, sizeof(pof));
-  if (e == cudaSuccess) e = cudaMemcpyToSymbol(g_dmc_pmask, pmask, sizeof(pmask));
-  if (e != cudaSuccess) g_dmc_tables_uploaded = 0;  // retry on the next call
-  return e;
-}
-
 DmcWS DmcWS::from(char* base, int G, int B, size_t* bytes) {
   char* p = base;
   DmcWS w;
@@ -419,14 +357,19 @@ cudaError_t launch_dmc_emit(int B, int G, const float* phi, float iso, void* ws,
   return cudaGetLastError();
 }
 
+void launch_dmc_first_vertex(int G, const McItems& it, const int32_t* vsrc, unsigned long long* cvid,
+                             cudaStream_t s) {
+  const int V = it.voff[it.B];
+  if (V > 0) dmc_first_vertex_kernel<<<(V + 255) / 256, 256, 0, s>>>((size_t)G * G * G, it, vsrc, cvid);
+}
+
 cudaError_t launch_dmc_backward(int G, const McItems& it, const float* phi, float iso, void* ws, const int32_t* vsrc,
                                 const float* dverts, float* dphi, cudaStream_t s) {
   cudaError_t e = upload_dmc_tables();
   if (e != cudaSuccess) return e;
   DmcWS w = DmcWS::from((char*)ws, G, it.B);
   const size_t G3 = (size_t)G * G * G, n = (size_t)it.B * G3;
-  const int V = it.voff[it.B];
-  if (V > 0) dmc_first_vertex_kernel<<<(V + 255) / 256, 256, 0, s>>>(G3, it, vsrc, w.cvid);
+  launch_dmc_first_vertex(G, it, vsrc, w.cvid, s);
   dmc_backward_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(G, it, phi, iso, w.cvid, dverts, dphi);
   return cudaGetLastError();
 }

@@ -58,6 +58,9 @@ cudaError_t launch_dmc_count(int B, int G, const float* phi, float iso, void* ws
 // verts[V_cap,3], vsrc[V_cap] = cell * 4 + patch (cell local to its item), faces[2 Q_cap, 3], quads[Q_cap, 4] or null
 cudaError_t launch_dmc_emit(int B, int G, const float* phi, float iso, void* ws, float* verts, int32_t* vsrc,
                             long long V_cap, int32_t* faces, int32_t* quads, long long Q_cap, cudaStream_t s);
+// cvid[cell] = the first dual vertex of every cell with one (item-local), rebuilt from vsrc
+void launch_dmc_first_vertex(int G, const McItems& it, const int32_t* vsrc, unsigned long long* cvid,
+                             cudaStream_t s);
 // ws: any workspace of the batch's size (the backward rebuilds the cells' first vertices from vsrc)
 cudaError_t launch_dmc_backward(int G, const McItems& it, const float* phi, float iso, void* ws, const int32_t* vsrc,
                                 const float* dverts, float* dphi, cudaStream_t s);

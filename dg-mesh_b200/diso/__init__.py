@@ -37,6 +37,15 @@ def _notifier(dev_index):
     return n
 
 
+def _remember_caps(key, cap, V, P, max_verts):
+    """The capacities the next call at `key` emits with: the counts V, P plus a quarter and 1024, never below the
+    previous capacities `cap`, V at most max_verts."""
+    if len(_caps) > 32:
+        _caps.clear()
+    _caps[key] = [min(max(cap[0] if cap else 0, int(V * 1.25) + 1024), max_verts),
+                  max(cap[1] if cap else 0, int(P * 1.25) + 1024)]
+
+
 class _Extractor:
     """The C entry points of one surface extractor.  Both count {V_k, P_k} per item (P: faces of marching cubes,
     quads of dual marching cubes), emit optimistically into caller capacities and map dL/dverts to dL/dphi; the
@@ -112,10 +121,7 @@ class _MCFunction(torch.autograd.Function):
         V, P = sum(c[0] for c in counts), sum(c[1] for c in counts)
         if out is None or V > cap[0] or P > cap[1] or (want_quads and out[3].shape[0] < P):
             out = emit(V, P)      # V beyond what the emission can index is refused there (DgmError)
-        if len(_caps) > 32:
-            _caps.clear()
-        _caps[key] = [min(max(cap[0] if cap else 0, int(V * 1.25) + 1024), kind.max_verts),
-                      max(cap[1] if cap else 0, int(P * 1.25) + 1024)]
+        _remember_caps(key, cap, V, P, kind.max_verts)
         verts, vsrc = out[0][:V], out[1][:V]
         faces, quads = out[2][:(2 * P if kind.dual else P)], out[3][:P]
         if not normalize:

@@ -942,6 +942,52 @@ int dgdmc_backward_batch(int B, int G, const int32_t* V_host, const float* phi, 
                          const int32_t* vsrc, const float* dL_dverts, float* dL_dphi, void* stream);
 
 /* ------------------------------------------------------------------------
+ * FlexiCubes (Shen et al. 2023; the extractor of nvdiffrec and kaolin) on the topology of dgdmc_*:
+ *   phi[G,G,G] fp32, iso, deform[G,G,G,3], alpha[G-1,G-1,G-1,8], beta[G-1,G-1,G-1,12], gamma_f[G-1,G-1,G-1]
+ *   ->  verts[V (+ Q),3] fp32 in [0,1]^3, faces[2Q (4Q),3] int32, L_dev per crossing
+ * Definition:
+ *   - Grid, corners, edges, cases, patches, "inside" (phi < iso) and which patches get a vertex are dgdmc_*'s, so
+ *     V and Q are what dgdmc_count returns; its workspace is the emission's.
+ *   - s = phi - iso; node n sits at x_n = n + deform[n] (grid units; NULL: 0).  The raw per-cell weights are
+ *     indexed by corner r = (i + (r&1), j + ((r>>1)&1), k + (r>>2)) and edge e = 4 axis + combo, and activated as
+ *     kaolin does: beta = 1 + 0.99 tanh(b), alpha = 1 + 0.99 tanh(a), gamma = 0.005 + 0.99 sigmoid(g); NULL is raw
+ *     0 (beta = alpha = 1, gamma = 1/2).
+ *   - Crossing on cut edge e, lower / upper corners r0 / r1: w0 = alpha[r0] s(n0), w1 = alpha[r1] s(n1),
+ *     t = w0 / (w0 - w1), u_e = x0 + t (x1 - x0).
+ *   - Dual vertex: (sum_e beta[e] u_e) / (sum_e beta[e]), summed in fp32 in increasing edge id, then / (G - 1).
+ *     With neutral weights, no deform and iso = 0 every operation rounds as dgdmc_*'s: the vertices are equal.
+ *   - Inference (training = 0): each quad (q0,q1,q2,q3) of dgdmc_emit, a vertex's gamma its cell's, gives
+ *     (q0,q1,q2), (q0,q2,q3) when gamma0 gamma2 >= gamma1 gamma3 (dgdmc's split), else (q0,q1,q3), (q1,q2,q3).
+ *   - Training (training = 1): quad q gets a centre vertex at row V + q, m = (g02 (v0+v2)/2 + g13 (v1+v3)/2) /
+ *     (g02 + g13 + 1e-8), g02 = gamma0 gamma2, g13 = gamma1 gamma3, and faces (q0,q1,m), (q1,q2,m), (q2,q3,m),
+ *     (q3,q0,m).
+ *   - L_dev: for each vertex v and each crossing of its patch, |d_e - mean_e d_e|, d_e = |u_e - v| in output units
+ *     (normalize = 1: / (G - 1)), written to ldev[v, slot] (slot: rank of e among the patch's edges, at most 7;
+ *     unused slots 0), with the crossing count in vk[v].
+ * dgfc_emit, after dgdmc_count on ws: verts[V_cap (+ Q_cap in training), 3], vsrc[V_cap] (as dgdmc_emit),
+ * ldev[V_cap, 7], vk[V_cap], faces[(2 | 4) Q_cap, 3], quads[Q_cap, 4] (dgdmc's oriented quads, read by the
+ * backward).  Capacities are enforced on the device, so it may be enqueued optimistically and re-run.
+ * Limits: as dgdmc_*; in training Q_cap < 2^29, so V + Q < 2^28 + 2^29 vertex indices and 4 Q < 2^31 triangles.
+ * dgfc_backward: dL_dverts[V (+ Q), 3] w.r.t. the normalised vertices and dL_dldev[V, 7] (or NULL) ->
+ * dL_dphi[G,G,G], and, each when not NULL, dL_ddeform[G,G,G,3], dL_dalpha, dL_dbeta, dL_dgamma (training only)
+ * w.r.t. the raw inputs, every element written (zero away from the surface).  verts, vsrc and quads are the
+ * emission's; V and Q are dgdmc_count's.  Nothing flows to iso; the gradient at |.| = 0 is 0.  Every gradient is
+ * gathered in a fixed order, without float atomics: bit-identical from run to run.  Its workspace is
+ * dgfc_backward_workspace_size(G, V, Q, training) bytes: dgdmc's plus 56 bytes per vertex, and 48 more per vertex
+ * and 64 per quad in training.  Bad arguments are refused on the host before any device work.
+ * ------------------------------------------------------------------------ */
+int dgfc_emit(int G, const float* phi, float iso, const float* deform, const float* alpha, const float* beta,
+              const float* gamma_f, int training, int normalize, void* ws, size_t ws_bytes, float* verts,
+              int32_t* vsrc, float* ldev, int32_t* vk, int64_t V_cap, int32_t* faces, int32_t* quads, int64_t Q_cap,
+              void* stream);
+int dgfc_backward_workspace_size(int G, int V, int Q, int training, size_t* bytes);
+int dgfc_backward(int G, int V, int Q, const float* phi, float iso, const float* deform, const float* alpha,
+                  const float* beta, const float* gamma_f, int training, int normalize, const float* verts,
+                  const int32_t* vsrc, const int32_t* quads, const float* dL_dverts, const float* dL_dldev, void* ws,
+                  size_t ws_bytes, float* dL_dphi, float* dL_ddeform, float* dL_dalpha, float* dL_dbeta,
+                  float* dL_dgamma, void* stream);
+
+/* ------------------------------------------------------------------------
  * Tensor-core GEMM building blocks of the MLPs (wgmma, bf16 operands, fp32 accumulation in
  * registers), exposed stand-alone for the parity tests (torch.matmul on the same bf16 operands is the
  * oracle).  The networks below drive the same two kernels on activations kept in the library's
