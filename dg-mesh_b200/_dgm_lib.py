@@ -259,6 +259,9 @@ SIGNATURES.update({
     "dgpm_forward": (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, P, c_size_t, P]),
     "dgpm_backward_workspace": _DGE_SIZE,
     "dgpm_backward": (c_int, [c_int, c_int, c_int, P, P, P, P, P, P, P, P, P, c_size_t, P]),
+    # winding: verts, faces, points, beta, winding, dist2, face, bary, ws, bytes
+    "dgpm_winding_workspace": _DGE_SIZE,
+    "dgpm_winding": (c_int, [c_int, c_int, c_int, P, P, P, c_float, P, P, P, P, P, c_size_t, P]),
 })
 
 # deformation regularisers: the graph (P, K, weight_lambda, points, index, dist2, weight, inv_offsets, inv_pairs, ws,

@@ -2283,6 +2283,29 @@ int dgpm_backward(int V, int F, int Q, const float* verts, const int32_t* faces,
                                                    grad_dist2, grad_points, grad_verts, ws, (cudaStream_t)stream));
 }
 
+int dgpm_winding_workspace(int V, int F, int Q, size_t* bytes) {
+  const int rc = dgpm_sizes("dgpm_winding_workspace", V, F, Q);
+  if (rc != DGM_OK) return rc;
+  if (!bytes) return bad("dgpm_winding_workspace: null pointer");
+  dgm::WnWS::from(nullptr, F, Q, dgm::pm_fwd_cub_bytes(F, Q), bytes);
+  return DGM_OK;
+}
+
+int dgpm_winding(int V, int F, int Q, const float* verts, const int32_t* faces, const float* points, float beta,
+                 float* winding, float* dist2, int64_t* face, float* bary, void* ws, size_t ws_bytes, void* stream) {
+  const int rc = dgpm_sizes("dgpm_winding", V, F, Q);
+  if (rc != DGM_OK) return rc;
+  if (!(beta > 0.f)) return bad("dgpm_winding: beta must be > 0 (+inf for the exact sum)");
+  if (Q == 0) return DGM_OK;
+  if (!verts || !faces || !points || !winding || !ws) return bad("dgpm_winding: null pointer");
+  if (!dist2 != !face || !dist2 != !bary) return bad("dgpm_winding: dist2, face and bary must be all NULL or none");
+  size_t need;
+  dgpm_winding_workspace(V, F, Q, &need);
+  if (ws_bytes < need) return dge_short("dgpm_winding", ws_bytes, need);
+  return check(dgm::launch_winding_number(F, Q, verts, faces, points, beta, winding, dist2, (long long*)face, bary,
+                                          ws, (cudaStream_t)stream));
+}
+
 // ---- deformation regularisers and their K-nearest-neighbour graph.  Every argument is checked here, before any
 // device work.
 namespace {

@@ -397,10 +397,8 @@ __global__ void __launch_bounds__(128) pm_query_kernel(int Q, int F, int L, cons
   bary[3 * (size_t)q + 2] = best.w;
 }
 
-cudaError_t launch_point_mesh_distance(int F, int Q, const float* verts, const int32_t* faces, const float* points,
-                                       float* dist2, long long* face, float* bary, void* ws, cudaStream_t s) {
-  if (Q == 0) return cudaSuccess;
-  PmFwdWS w = PmFwdWS::from((char*)ws, F, Q, pm_fwd_cub_bytes(F, Q));
+void pm_build(int F, int Q, const float* verts, const int32_t* faces, const float* points, const PmFwdWS& w,
+              cudaStream_t s) {
   const int L = (F + PM_LEAF - 1) / PM_LEAF;
   cudaMemsetAsync(w.bounds, 0, 8 * sizeof(uint32_t), s);
   cudaMemsetAsync(w.qbounds, 0, 8 * sizeof(uint32_t), s);
@@ -417,8 +415,21 @@ cudaError_t launch_point_mesh_distance(int F, int Q, const float* verts, const i
   knn_morton_kernel<<<(Q + 255) / 256, 256, 0, s>>>(Q, points, w.qbounds, w.qcodes, w.qidx);
   tb = w.cub_bytes;
   cub::DeviceRadixSort::SortPairs(w.cub_temp, tb, w.qcodes, w.qcodes_sorted, w.qidx, w.qorder, Q, 0, 30, s);
+}
+
+void pm_query(int F, int Q, const float* points, const PmFwdWS& w, float* dist2, long long* face, float* bary,
+              cudaStream_t s) {
+  const int L = (F + PM_LEAF - 1) / PM_LEAF;
   pm_query_kernel<<<(Q + 127) / 128, 128, 0, s>>>(Q, F, L, points, w.qorder, (const float4*)w.tri, w.nodes, dist2,
                                                   face, bary);
+}
+
+cudaError_t launch_point_mesh_distance(int F, int Q, const float* verts, const int32_t* faces, const float* points,
+                                       float* dist2, long long* face, float* bary, void* ws, cudaStream_t s) {
+  if (Q == 0) return cudaSuccess;
+  const PmFwdWS w = PmFwdWS::from((char*)ws, F, Q, pm_fwd_cub_bytes(F, Q));
+  pm_build(F, Q, verts, faces, points, w, s);
+  pm_query(F, Q, points, w, dist2, face, bary, s);
   return cudaGetLastError();
 }
 

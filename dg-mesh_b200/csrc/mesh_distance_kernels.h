@@ -33,6 +33,29 @@ struct PmFwdWS {
   static PmFwdWS from(char* base, size_t F, size_t Q, size_t cub_bytes, size_t* bytes = nullptr);
 };
 size_t pm_fwd_cub_bytes(int F, int Q);
+// the BVH over the faces and the queries' Morton order, into w (Q >= 1); then the closest-point query on them
+void pm_build(int F, int Q, const float* verts, const int32_t* faces, const float* points, const PmFwdWS& w,
+              cudaStream_t s);
+void pm_query(int F, int Q, const float* points, const PmFwdWS& w, float* dist2, long long* face, float* bary,
+              cudaStream_t s);
+
+// Barill et al. 2018's order-1 expansions of both children of one internal node (parallel to PmNode): centroid p~
+// and radius r, zeroth moment N = sum a_t n_t and total area A, first moment M = sum a_t (x_t - p~) n_t^T (row
+// major), and the children again, so a winding visit reads this record alone
+struct alignas(16) WnNode {
+  float4 pr[2];     // [child] p~ xyz, r
+  float4 na[2];     // [child] N xyz, A
+  float m[2][9];    // [child] M
+  int child[2];     // as PmNode::child
+};
+
+// winding number: the forward's BVH and query order, then the expansions with their own refit arrivals
+struct WnWS {
+  PmFwdWS pm;
+  WnNode* nodes;    // [L-1]
+  int* counter;     // [L-1]
+  static WnWS from(char* base, size_t F, size_t Q, size_t cub_bytes, size_t* bytes = nullptr);
+};
 
 // backward: the CSR inverse of the 3Q (vertex, entry) pairs
 struct PmBwdWS {
@@ -45,6 +68,10 @@ size_t pm_bwd_cub_bytes(int V, int Q);
 
 cudaError_t launch_point_mesh_distance(int F, int Q, const float* verts, const int32_t* faces, const float* points,
                                        float* dist2, long long* face, float* bary, void* ws, cudaStream_t s);
+// winding [Q] and, when dist2 is not null, launch_point_mesh_distance's outputs from the same build (ws: WnWS)
+cudaError_t launch_winding_number(int F, int Q, const float* verts, const int32_t* faces, const float* points,
+                                  float beta, float* winding, float* dist2, long long* face, float* bary, void* ws,
+                                  cudaStream_t s);
 cudaError_t launch_point_mesh_distance_bwd(int V, int Q, const float* verts, const int32_t* faces,
                                            const float* points, const long long* face, const float* bary,
                                            const float* grad_dist2, float* grad_points, float* grad_verts, void* ws,

@@ -1,5 +1,6 @@
 """Mesh-to-mesh metrics of DG-Mesh's evaluation: Chamfer distance and the approximate EMD between surface samples
-(PointFlow's `cd` and `emd_approx`, on metrics.pytorch_structural_losses), plus F-score and normal consistency.
+(PointFlow's `cd` and `emd_approx`, on metrics.pytorch_structural_losses), plus F-score, normal consistency and,
+optionally, volumetric IoU.
 
 Meshes are (verts [V,3], faces [F,3]) in the caller's units: nothing is normalised, aligned or cleaned.  Sampling is
 plain torch (it is not a hot path); the distances, the closest points on a surface and the matching run on this
@@ -15,7 +16,7 @@ if _root not in sys.path:
     sys.path.insert(0, _root)
 from metrics.pytorch_structural_losses.match_cost import match_cost  # noqa: E402
 from metrics.pytorch_structural_losses.nn_distance import nn_distance_with_indices  # noqa: E402
-from mesh_distance import point_mesh_distance  # noqa: E402
+from mesh_distance import point_mesh_distance, winding_number  # noqa: E402
 
 
 def sample_surface(verts, faces, n, generator=None):
@@ -67,7 +68,7 @@ def _face_normals(verts, faces):
     return torch.nn.functional.normalize(torch.linalg.cross(b - a, c - a), dim=1)
 
 
-def mesh_metrics(pred, gt, n_points, thresholds=(), generator=None, surface=False):
+def mesh_metrics(pred, gt, n_points, thresholds=(), generator=None, surface=False, iou_points=0):
     """Sample n_points on each mesh (sample_surface, pred first) and compare the samples.
 
     pred, gt: (verts [V,3], faces [F,3]); the samples go to the device of pred's verts, which must be CUDA.
@@ -83,7 +84,16 @@ def mesh_metrics(pred, gt, n_points, thresholds=(), generator=None, surface=Fals
     points) instead of against its samples: dist1 / dist2 above become squared point-to-mesh distances, so the
     sampling noise of the other mesh drops out (a mesh against itself scores 0 up to rounding), and
     normal_consistency takes the normal of the closest face.  The samples are drawn with the same calls in the same
-    order in both modes, so with the same generator both measure the same points; emd is the same in both."""
+    order in both modes, so with the same generator both measure the same points; emd is the same in both.
+
+    With iou_points > 0 the dict also has iou = |inside_pred and inside_gt| / |inside_pred or inside_gt| (0.0 when
+    no point is inside either mesh) over iou_points points uniform in the union of the two meshes' axis-aligned
+    boxes, drawn with the same generator after the surface samples, so every other entry is the same as with
+    iou_points = 0.  A point is inside a mesh when |winding_number| >= 0.5 (beta = 2): right for closed meshes of
+    either consistent orientation, graceful on open ones.  Its standard error is about sqrt(iou (1 - iou) / n_in),
+    n_in the points inside either mesh."""
+    if isinstance(iou_points, bool) or not isinstance(iou_points, int) or iou_points < 0:
+        raise ValueError("mesh_metrics: iou_points must be an int >= 0")
     pv, pf = _mesh(pred, "pred")
     gv, gf = _mesh(gt, "gt")
     p, _, pn = sample_surface(pv, pf, n_points, generator)
@@ -110,4 +120,20 @@ def mesh_metrics(pred, gt, n_points, thresholds=(), generator=None, surface=Fals
         P, R = float((s1 < tau).double().mean()), float((s2 < tau).double().mean())
         out["precision"][tau], out["recall"][tau] = P, R
         out["fscore"][tau] = 2 * P * R / (P + R) if P + R > 0 else 0.0
+    if iou_points > 0:
+        out["iou"] = _iou(pv, pf, gv, gf, iou_points, generator)
     return out
+
+
+def _iou(pv, pf, gv, gf, n, generator):
+    dev = pv.device
+    pv32, gv32 = pv.detach().to(dev, torch.float32), gv.detach().to(dev, torch.float32)
+    lo = torch.minimum(pv32.min(0).values, gv32.min(0).values).double()
+    hi = torch.maximum(pv32.max(0).values, gv32.max(0).values).double()
+    rdev = generator.device if generator is not None else dev
+    r = torch.rand(n, 3, dtype=torch.float64, generator=generator, device=rdev).to(dev)
+    x = (lo + (hi - lo) * r).float().contiguous()
+    a = winding_number(x, pv32, pf.to(dev)).abs() >= 0.5
+    b = winding_number(x, gv32, gf.to(dev)).abs() >= 0.5
+    union = int((a | b).sum())
+    return int((a & b).sum()) / union if union > 0 else 0.0

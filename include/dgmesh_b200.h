@@ -1445,6 +1445,27 @@ int dgpm_backward(int V, int F, int Q, const float* verts, const int32_t* faces,
                   const int64_t* face, const float* bary, const float* grad_dist2, float* grad_points,
                   float* grad_verts, void* ws, size_t ws_bytes, void* stream);
 
+/* dgpm_winding: the generalized winding number (Jacobson et al. 2013) of the mesh at every query q,
+ *   winding[q] = (1 / 4 pi) sum over faces f of Omega_f(q),
+ *   Omega_f(q) = 2 atan2(det[a b c], |a||b||c| + (a.b)|c| + (b.c)|a| + (c.a)|b|), a, b, c = the face's vertices
+ *   in the order faces[f][0..2], minus points[q],
+ * with Omega_f(q) = 0 where det[a b c] is exactly 0 (a query on a face, edge or vertex, and faces with coincident
+ * or collinear vertices add nothing).  Orientation: winding = +1 inside a closed mesh whose faces are
+ * counter-clockwise seen from outside (right-hand normal (b - a) x (c - a) pointing out), -1 inside one oriented
+ * the other way, 0 outside; open, non-manifold or self-intersecting meshes give values in between that degrade
+ * smoothly.  The sum is evaluated on dgpm_forward's BVH with Barill et al. 2018's order-1 expansion of every child
+ * cluster (area-weighted centroid p~, radius r bounding its vertices): a cluster with |points[q] - p~| > beta r
+ * adds its far-field term instead of its faces.  beta > 0 and not NaN; beta = +inf never takes the far field and
+ * gives the exact sum of the fp32 solid angles (accumulated in float64).  The result is bit-identical from run to
+ * run and does not depend on the other queries of the call.
+ * dist2, face and bary are all NULL (winding only) or all non-NULL: then they are dgpm_forward's outputs, bit for
+ * bit, from the same build.  DGM_E_BADARG also for beta <= 0 or NaN, or for only some of dist2, face, bary NULL.
+ * Workspace: dgpm_winding_workspace (depends on F and Q; dgpm_forward's plus the expansions).
+ * ------------------------------------------------------------------------ */
+int dgpm_winding_workspace(int V, int F, int Q, size_t* bytes);
+int dgpm_winding(int V, int F, int Q, const float* verts, const int32_t* faces, const float* points, float beta,
+                 float* winding, float* dist2, int64_t* face, float* bary, void* ws, size_t ws_bytes, void* stream);
+
 /* ------------------------------------------------------------------------
  * Deformation regularisers (Dynamic 3D Gaussians' local rigidity, rotation similarity and isometry) over an exact
  * K-nearest-neighbour graph of the Gaussians.  All pointers are device memory.  Nothing allocates or synchronises
